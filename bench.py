@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- local-aggregation hot path: points/s (forward + backward) on N B200s.
+"""bench.py -- local-aggregation hot path: points/s (forward + backward) on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config 1..5] [--impl ours|reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -9,7 +9,7 @@ One "step" = one LocalAggregation call of the BASELINE.json configuration (defau
 single-GPU configuration: S3DIS Pseudo-Grid, B=8 N=15000 K=26 C=72 per GPU), forward AND backward (gradients w.r.t. the input
 features and every parameter), INCLUDING the neighbour search (the neighbour-list cache is disabled, so no
 step re-uses the previous step's search), on a fresh synthetic batch: a ring of pre-generated batches larger
-than the 126 MB L2 is rotated so that no step finds its inputs in L2.  Multi-GPU: batches shard over ranks
+than the 50 MB L2 is rotated so that no step finds its inputs in L2.  Multi-GPU: batches shard over ranks
 (weak scaling: B per GPU is fixed), the only exchange is the NCCL all-reduce of parameter gradients, captured in
 the step's CUDA graph.  The other four BASELINE configurations are measured the same way (device-timed) and
 reported under "configs" in the same JSON line (c4/c5 at their per-GPU shard: B/8 clouds per GPU).
@@ -59,6 +59,9 @@ def parse():
     ap.add_argument("--no-ref-gpu", action="store_true")
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-e2e", action="store_true", help="skip the end-to-end leg (profiling captures: keeps the run to 3 steps)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (output, d/dfeatures, "
+                         "parameter gradients) as DIR/<name>.npy, float32, at most 64 MB in all")
     return ap.parse_args()
 
 
@@ -67,7 +70,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 class ClockSampler:
@@ -204,6 +207,35 @@ def algo_bytes_per_point(name, C, K, Cout):
     return table.get(name)
 
 
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write {name: tensor} as out_dir/<name>.npy in float32.  Arrays that fit the budget are written whole (smallest
+    first); each remaining array gets an equal share of what is left and is written as a fixed sample of its
+    flattened elements (indices drawn once from a generator seeded with 0, sorted), so that two builds given the same
+    arguments can be compared element for element."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    items = sorted(arrays.items(), key=lambda kv: kv[1].numel())
+    left = (DUMP_BUDGET_BYTES - 4096 * len(items)) // 4   # room for the .npy headers
+    written = {}
+    for i, (name, t) in enumerate(items):
+        flat = t.detach().float().reshape(-1)
+        share = left // (len(items) - i)
+        if flat.numel() > share:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(flat.numel(), generator=g)[:share].sort().values
+            flat = flat[idx.to(flat.device)]
+            written[name] = f"sample of {share} of {t.numel()} elements, shape {list(t.shape)}"
+        else:
+            flat = flat.reshape(t.shape)
+            written[name] = f"shape {list(t.shape)}"
+        left -= flat.numel()
+        np.save(os.path.join(out_dir, name + ".npy"), flat.cpu().numpy().astype(np.float32))
+    return written
+
+
 def build_module(spec, device):
     import numpy as np
     from closerlook3d_b200.local_aggregation_operators import LocalAggregation
@@ -279,7 +311,7 @@ def local_batch(args, spec):
 
 
 def device_leg(spec, B_local, rank, world, device, steps, warmup, use_graph=True, sampler=None, want_profile=False,
-               keep=False):
+               keep=False, dump_dir=None):
     """Device-timed leg of one configuration: `warmup` untimed steps, then exactly `steps` steps between
     (barrier + synchronize) brackets, timed with CUDA events on the launch stream; MAX over ranks.
     Inputs are resident in HBM (a ring of batches larger than L2) when the timed region starts."""
@@ -290,7 +322,7 @@ def device_leg(spec, B_local, rank, world, device, steps, warmup, use_graph=True
     pt_utils.clear_neighbor_cache()
     mod, radius = build_module(spec, device)
     mod.train()
-    L2 = 126e6
+    L2 = 50e6
     ring = make_ring(spec, B_local, rank, device, 1.6 * L2)
     C, N, K = spec["C"], spec["N"], spec["K"]
     gout = torch.randn(B_local, C, N, device=device, generator=torch.Generator(device=device).manual_seed(5))
@@ -327,6 +359,17 @@ def device_leg(spec, B_local, rank, world, device, steps, warmup, use_graph=True
             return gs.replay()
         return eager_step(batch)
 
+    def last_step_arrays(out, batch):
+        """what a caller of the step receives: the output, d/dfeatures and the parameter gradients"""
+        if use_graph:
+            f_grad, grads = gs.features.grad, gs.grads()
+        else:
+            f_grad, grads = batch["features"].grad, [p.grad for p in params if p.requires_grad]
+        names = [n for n, p in mod.named_parameters() if p.requires_grad]
+        arrays = {"out": out, "grad_features": f_grad}
+        arrays.update({"grad_" + n: g for n, g in zip(names, grads) if g is not None})
+        return arrays
+
     # kernels of one step (a graph replay does not pass through the library's launch counter: count one eager step)
     torch.cuda.synchronize()
     c0 = L.cl3d_launch_count()
@@ -354,13 +397,14 @@ def device_leg(spec, B_local, rank, world, device, steps, warmup, use_graph=True
     for s in range(steps):
         b = ring[(warmup + s) % len(ring)]
         ev[s][0].record()
-        step(b)
+        out = step(b)
         ev[s][1].record()
     e_all1.record()
     torch.cuda.synchronize()
     t_wall = time.perf_counter() - t_wall0
     if sampler is not None:
         sampler.mark_stop()
+    dumped = dump_outputs(dump_dir, last_step_arrays(out, b)) if dump_dir and rank == 0 and steps > 0 else None
     if world > 1:
         dist.barrier()
     total_ms = e_all0.elapsed_time(e_all1)
@@ -374,6 +418,8 @@ def device_leg(spec, B_local, rank, world, device, steps, warmup, use_graph=True
     res = dict(value=pts_per_step / (ms_per_step * 1e-3), ms_per_step=ms_per_step, ms_per_step_median=med_ms,
                launches=per_step * steps, launches_per_step=per_step, B_local=B_local, wall_s=t_wall,
                points_per_step=pts_per_step, radius=radius)
+    if dumped is not None:
+        res["dumped"] = dumped
 
     # ---- per-entry-point device time (separate identical pass, CUDA events on the launch stream, eager: the
     #      events need the library calls, not a graph replay)
@@ -407,7 +453,7 @@ def e2e_leg(args, spec, res, rank, world, device):
     with numa_local(device) as nl:
         hring = make_ring(spec, B_local, rank, device, 0.0, pinned=True)
         h2d = sum(v.numel() * v.element_size() for v in hring[0].values())
-        nst = max(args.steps, 100)   # short windows are dominated by host jitter
+        nst = args.steps
         # the host link on its own: one batch, pinned -> device, 10 back-to-back copies (the e2e rate cannot exceed
         # points_per_batch / this time; the link is shared with the other tenants of the box)
         dbuf = {k: torch.empty_like(v, device=device) for k, v in hring[0].items()}
@@ -601,7 +647,7 @@ def ref_gpu_arm(spec, device, res):
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / n
         return {"value": B * N / (ms * 1e-3), "unit": "points/s", "ms_per_step": ms, "parity": parity,
-                "what": "reference CUDA ext (sm_100, unmodified) + unfused python layer, 1 GPU, fwd+bwd"}
+                "what": "reference CUDA ext (sm_90, unmodified) + unfused python layer, 1 GPU, fwd+bwd"}
     except Exception as e:  # e.g. out of memory on the inflated tensors
         return {"unavailable": str(e)[:200]}
 
@@ -610,7 +656,7 @@ def config_dict(workload, spec, B_local, world):
     """identical for both arms (the driver compares the two lines' `config`); how each arm runs is in `method`"""
     return {"workload": workload, "family": spec["la"], "clouds_per_gpu": B_local,
             "points_per_step": B_local * spec["N"] * world, "parallelism": f"dp{world}",
-            "l2": "GPU arm: inputs rotate over a ring of pre-generated batches > 1.6x L2 (126 MB), no step finds its "
+            "l2": "GPU arm: inputs rotate over a ring of pre-generated batches > 1.6x L2 (50 MB), no step finds its "
                   "inputs in L2"}
 
 
@@ -689,7 +735,7 @@ def main():
     sampler = ClockSampler(torch.cuda.current_device()).start()   # steady state long before the timed region
     B_local = local_batch(args, spec)
     res = device_leg(spec, B_local, rank, world, device, args.steps, args.warmup, use_graph=not args.no_graph,
-                     sampler=sampler, want_profile=True, keep=True)
+                     sampler=sampler, want_profile=True, keep=True, dump_dir=args.dump_outputs)
     clocks = sampler.stop()
     trace(f"device leg done: {res['ms_per_step']:.4f} ms/step")
     e2e = None if args.no_e2e else e2e_leg(args, spec, res, rank, world, device)
@@ -703,7 +749,7 @@ def main():
                 continue
             sp = baseline_config(ci)
             Bl = sp["B"] if sp["gpus"] == 1 else max(1, sp["B"] // sp["gpus"])
-            st = max(10, min(args.steps, 30))
+            st = min(args.steps, 30)
             try:
                 r = device_leg(sp, Bl, rank, world, device, st, max(3, min(args.warmup, 5)),
                                use_graph=not args.no_graph)
@@ -738,7 +784,7 @@ def main():
     step_bytes = step_algo_bytes_per_point(C, K) * pts_local
     if kern:
         top = kern[0]
-        # DRAM bytes per launch of the same entry point from the committed `ncu --set full` capture of this workload
+        # DRAM bytes per launch of the same entry point from an `ncu --set full` capture of this workload
         # (profiles/traffic.json, written by tools/ncu_traffic.py); null when no capture exists for the config
         traffic, traffic_src = None, None
         tp = os.path.join(ROOT, "profiles", "traffic.json")
@@ -779,7 +825,7 @@ def main():
                        "timing": "CUDA events around the K steps, (barrier + synchronize) on both sides, max over ranks",
                        "neighbour_cache": "disabled (search runs every step)"},
             "clocks": clocks, "gpu_launches": res["launches"], "gpu_launches_per_step": res["launches_per_step"],
-            "e2e": e2e, "roofline": roof, "cpu_baseline": cb, "kernels": kern[:8], "configs": extra, "ref_gpu": rg}
+            "dumped_outputs": res.get("dumped"), "e2e": e2e, "roofline": roof, "cpu_baseline": cb, "kernels": kern[:8], "configs": extra, "ref_gpu": rg}
     print(json.dumps(line), file=real_stdout, flush=True)
     trace("line printed")
     shutdown_distributed(world, res)

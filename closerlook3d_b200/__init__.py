@@ -1,4 +1,4 @@
-"""closerlook3d_b200 -- Blackwell-native (sm_100a) local-aggregation engine, drop-in for the hot path of
+"""closerlook3d_b200 -- H100-native (Hopper, sm_90a) local-aggregation engine, drop-in for the hot path of
 zeliu98/CloserLook3D (see DESIGN.md).  Public surface mirrors the reference:
 
     closerlook3d_b200.local_aggregation_operators   LocalAggregation, PosPool, AdaptiveWeight, PointWiseMLP, PseudoGrid

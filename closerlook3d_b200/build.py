@@ -1,8 +1,8 @@
-"""Build libcl3d.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libcl3d.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m closerlook3d_b200.build [--force]
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with the snapshot.
+nvcc cross-compiles without a GPU.  The .so and the objects are build products (git-ignored).
 """
 import os
 import subprocess
@@ -14,7 +14,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 SO_PATH = os.path.join(PKG_DIR, "libcl3d.so")
 OBJ_DIR = os.path.join(PKG_DIR, "csrc", "_obj")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--expt-relaxed-constexpr", "--extended-lambda", "-Xcompiler", "-fPIC"]
 
 
@@ -60,7 +60,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=max(1, min(8, len(cmds) or 1))) as ex:
         list(ex.map(run, cmds))
-    run([nvcc, "-shared", "-o", SO_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+    run([nvcc, "-shared", "-o", SO_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return SO_PATH
 
 

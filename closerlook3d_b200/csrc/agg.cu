@@ -1,5 +1,5 @@
 // agg.cu -- fused local aggregation, forward and backward, for the per-(channel, neighbour)-weight families
-//           PosPool(xyz | sin_cos), AdaptiveWeight(dp) and PseudoGrid (sm_100a).
+//           PosPool(xyz | sin_cos), AdaptiveWeight(dp) and PseudoGrid (sm_90a).
 //
 // Replaces, per LocalAggregation call of the reference
 //   /root/reference/pytorch/ops/pt_custom_ops/pt_utils.py:121-144            (2x group_points, subtract, normalise)
@@ -19,9 +19,8 @@
 //   rows of d(loss)/d(agg) are streamed the same way; no float atomics on activations; parameter gradients
 //   are accumulated per CTA and reduced afterwards in a fixed order.
 //
-// r1a staged the rows with one cp.async.bulk (TMA) per row; ncu showed that design issue-bound (UBLKCP is a
-// uniform instruction: ~11 warp-instructions per 288-byte row, plus the LDS to read it back), 3-5x slower than
-// this version.  See profiles/r1a_pwmlp_fwd_tma_summary.md.
+// Staging the rows with one cp.async.bulk (TMA) per row makes the kernel issue-bound (about 11 warp-instructions
+// per 288-byte row, plus the shared-memory load to read it back); plain coalesced loads do better here.
 #include "agg_common.cuh"
 
 namespace cl3d {
@@ -571,9 +570,9 @@ __device__ __forceinline__ float div_by(float n, float d, float rcp_d) {
   return q;
 }
 
-// sin and cos of two arguments at once (the same wave length for two neighbour slots).  ncu on the polynomial version
-// (profiles/r2h_sincos_summary.md): 34 instructions per (neighbour, wave length) evaluation, issue-bound, 10 of them
-// packed polynomial steps and 8 the quadrant swap / sign logic.  Here the argument is reduced EXACTLY (Cody-Waite with
+// sin and cos of two arguments at once (the same wave length for two neighbour slots).  A polynomial version needs
+// about 34 instructions per (neighbour, wave length) evaluation, most of them polynomial steps and quadrant swap /
+// sign logic.  Here the argument is reduced EXACTLY (Cody-Waite with
 // a three-term 2*pi, packed; the nearest integer by the magic-number add, no F2I / FRND) to r in [-pi, pi], where the
 // hardware approximations are specified to 2^-21.4 (sin) / 2^-21.2 (cos) absolute error -- 4e-7, with the averaging over
 // the K neighbours well inside the 1e-5 parity bar (measured in tests/test_local_aggregation_gpu.py) -- and cost one
@@ -606,7 +605,7 @@ __device__ __forceinline__ void consume_pairs(const float* __restrict__ base, co
   }
   const u64 hundred = pack2(100.f, 100.f);
   // The gathered values of slot pair s+2 are requested BEFORE the arithmetic of slot pair s (software pipeline, one
-  // pair deep): in the r2h profile a third of the stall samples sat on the accumulate FFMA2s waiting for loads that
+  // pair deep): a third of the stall samples sat on the accumulate FMAs waiting for loads that
   // had been issued ~45 instructions earlier -- an L2 hit takes several hundred cycles.
   auto gather = [&](int s0, u64 (&vs2)[PI], u64 (&vc2)[PI]) {
     const unsigned o0 = __float_as_uint(s_dp[s0].w), o1 = __float_as_uint(s_dp[s0 + 1].w);   // row element offsets

@@ -1,4 +1,4 @@
-// agg_max.cu -- fused local aggregation with MAX reduction for PosPool (xyz | sin_cos) and AdaptiveWeight (sm_100a).
+// agg_max.cu -- fused local aggregation with MAX reduction for PosPool (xyz | sin_cos) and AdaptiveWeight (sm_90a).
 //
 // Replaces /root/reference/pytorch/models/local_aggregation_operators.py:87-91 (PosPool) and :199-203
 // (AdaptiveWeight): F.max_pool2d over the nsample axis of the (B,C,npoint,nsample) product tensor, and its

@@ -1,5 +1,5 @@
 // bn.cu -- the out_transform of PosPool / AdaptiveWeight / PseudoGrid: BatchNorm1d + ReLU on the
-//          channel-major aggregated tensor (B,C,M), forward and backward (sm_100a).
+//          channel-major aggregated tensor (B,C,M), forward and backward (sm_90a).
 //
 // Replaces nn.Sequential(nn.BatchNorm1d(C, momentum), nn.ReLU(inplace=True)) of
 //   /root/reference/pytorch/models/local_aggregation_operators.py:43-45,110 (and :166-168, :363-365).

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libcl3d (sm_100a only).
+// common.cuh -- shared device/host helpers for libcl3d (sm_90a only).
 #pragma once
 #include <atomic>
 #include <cuda_runtime.h>
@@ -7,14 +7,14 @@
 
 #include "../../include/cl3d.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libcl3d is written for sm_100a (Blackwell) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libcl3d is written for sm_90a (Hopper) only"
 #endif
 
 namespace cl3d {
 
 constexpr int kWarp = 32;
-constexpr int kNumSMsFallback = 148;
+constexpr int kNumSMsFallback = 132;
 
 // ---------------------------------------------------------------------------------------------
 // error reporting (thread-local message, integer return codes; never exit())
@@ -105,8 +105,9 @@ __device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long v)
   return v;
 }
 
-// ---- packed fp32x2 arithmetic (Blackwell: FFMA2 / FMUL2 / FADD2).  A register-operand FFMA issues every other
-// cycle per scheduler; the packed forms carry two IEEE operations in the same slot.
+// ---- fp32 pairs.  Hopper has no packed fp32x2 instructions, so each pair operation is two IEEE-rounded scalar
+// operations (__fmaf_rn / __fmul_rn / ... are never contracted or reassociated by the compiler); the results are
+// the same bits a packed instruction gives.  A pair travels as one 64-bit value (lo = .x, hi = .y).
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 pack2(float lo, float hi) {
   u64 r;
@@ -117,24 +118,24 @@ __device__ __forceinline__ void unpack2(u64 v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-  u64 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-  u64 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ u64 add2(u64 a, u64 b) {
-  u64 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ u64 sub2(u64 a, u64 b) {  // a - b, component-wise (exactly rounded like __fsub_rn)
-  u64 d;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
 }
 
 __device__ __forceinline__ float sqrt_approx(float x) {  // MUFU: 2^-22 relative, sqrt(0) = 0
@@ -143,36 +144,28 @@ __device__ __forceinline__ float sqrt_approx(float x) {  // MUFU: 2^-22 relative
   return y;
 }
 __device__ __forceinline__ u64 fma2_bcast(float h, u64 b, u64 c) {  // (h, h) * b + c ; h is a scalar-broadcast operand
-  u64 d;
-  asm("{\n.reg .b64 hh;\nmov.b64 hh, {%1, %1};\nfma.rn.f32x2 %0, hh, %2, %3;\n}" : "=l"(d) : "f"(h), "l"(b), "l"(c));
-  return d;
+  float b0, b1, c0, c1;
+  unpack2(b, b0, b1); unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(h, b0, c0), __fmaf_rn(h, b1, c1));
 }
 
-// The same operations on plain float operands (32-bit "f" constraints).  ptxas then allocates the register pairs
-// itself and keeps loop-carried accumulators in place; with 64-bit "l" operands it computed into the freshly loaded
-// pair and copied the result back with four MOVs per step (profiles/r2e).
+// The same operations on plain float operands.
 //   (cx, cy) += (h, h) * (bx, by)
 __device__ __forceinline__ void ffma2_bcast(float h, float bx, float by, float& cx, float& cy) {
-  asm("{\n.reg .b64 a, b, hh;\nmov.b64 a, {%0, %1};\nmov.b64 b, {%3, %4};\nmov.b64 hh, {%2, %2};\n"
-      "fma.rn.f32x2 a, hh, b, a;\nmov.b64 {%0, %1}, a;\n}"
-      : "+f"(cx), "+f"(cy)
-      : "f"(h), "f"(bx), "f"(by));
+  cx = __fmaf_rn(h, bx, cx);
+  cy = __fmaf_rn(h, by, cy);
 }
 //   (cx, cy) += (ax, ay) * (bx, by)
 __device__ __forceinline__ void ffma2(float ax, float ay, float bx, float by, float& cx, float& cy) {
-  asm("{\n.reg .b64 a, b, c;\nmov.b64 a, {%2, %3};\nmov.b64 b, {%4, %5};\nmov.b64 c, {%0, %1};\n"
-      "fma.rn.f32x2 c, a, b, c;\nmov.b64 {%0, %1}, c;\n}"
-      : "+f"(cx), "+f"(cy)
-      : "f"(ax), "f"(ay), "f"(bx), "f"(by));
+  cx = __fmaf_rn(ax, bx, cx);
+  cy = __fmaf_rn(ay, by, cy);
 }
 //   (cx, cy) = (ax, ay) * (bx, by)
 __device__ __forceinline__ void fmul2(float ax, float ay, float bx, float by, float& cx, float& cy) {
-  asm("{\n.reg .b64 a, b, c;\nmov.b64 a, {%2, %3};\nmov.b64 b, {%4, %5};\n"
-      "mul.rn.f32x2 c, a, b;\nmov.b64 {%0, %1}, c;\n}"
-      : "=f"(cx), "=f"(cy)
-      : "f"(ax), "f"(ay), "f"(bx), "f"(by));
+  cx = __fmul_rn(ax, bx);
+  cy = __fmul_rn(ay, by);
 }
-// ---- mbarrier helpers (producer/consumer rings of the tcgen05 GEMM, gemm_tc.cuh) ----------
+// ---- mbarrier helpers (producer/consumer rings of the wgmma GEMM, gemm_tc.cuh) ----------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

@@ -1,4 +1,4 @@
-// gemm.cu -- fp32 GEMM with arbitrary element strides and optional split-K (sm_100a).
+// gemm.cu -- fp32 GEMM with arbitrary element strides and optional split-K (sm_90a).
 //
 // Used for the per-point products of the fused PointWiseMLP (see pwmlp.cu): the reference's per-neighbour
 // 1x1 conv over [dp; f_i; f_j - f_i] (/root/reference/pytorch/models/local_aggregation_operators.py:254-257,
@@ -7,7 +7,7 @@
 //   C[m][n] = sum_k A[m*sa_m + k*sa_k] * B[k*sb_k + n*sb_n]
 //
 // Two implementations behind cl3d_sgemm_algo:
-//   CL3D_GEMM_TC3X (default): tcgen05 tensor cores, every operand split into two TF32 halves and three MMAs
+//   CL3D_GEMM_TC3X (default): wgmma tensor cores, every operand split into two TF32 halves and three MMAs
 //     per product (gemm_tc.cuh) -- fp32-level accuracy, within the 1e-5 parity bar (BASELINE.json north_star);
 //   CL3D_GEMM_FFMA: the vectorised fp32 FMA kernel below (plain TF32/BF16 would break the parity bar).
 //
@@ -261,9 +261,8 @@ static int sgemm_ffma(const float* a, long long sa_m, long long sa_k, const floa
 
 // staged floats per k of one problem orientation: (#row tiles) x (#column tiles) x (128 + columns per tile)
 static long long tc_cost(int M, int N) {
-  const int nt = ceil_div(N, 256);
-  const int bn = N >= 256 ? 256 : ((N + 15) & ~15);
-  return (long long)ceil_div(M, kTcBM) * nt * (kTcBM + bn);
+  const int nt = ceil_div(N, kTcMaxN);
+  return (long long)ceil_div(M, kTcBM) * nt * (kTcBM + tc_tile_n(N));
 }
 
 static int sgemm_tc(const float* a, long long sa_m, long long sa_k, const float* b, long long sb_k, long long sb_n,
@@ -316,9 +315,9 @@ extern "C" int cl3d_sgemm_algo(const float* a, long long sa_m, long long sa_k, c
     }
     partial = (float*)workspace;
   }
-  // The tensor core accumulates with truncation (about half an ulp of bias per accumulation step, measured),
-  // so its error grows linearly with the k extent of one accumulator: AUTO keeps it to k ranges <= 512 per
-  // split (error ~1e-6 of the result) and leaves longer un-split reductions to the FMA kernel.
+  // AUTO leaves un-split reductions longer than 512 to the FMA kernel; the tensor-core kernel bounds the
+  // truncation of its accumulators by promoting them every 64 k (gemm_tc.cuh), so CL3D_GEMM_TC3X stays within
+  // the fp32 bar there too.
   if (algo == CL3D_GEMM_AUTO && ceil_div(K, splitk) > 512) algo = CL3D_GEMM_FFMA;
   if (algo != CL3D_GEMM_FFMA) {
     const int rc = sgemm_tc(a, sa_m, sa_k, b, sb_k, sb_n, M, N, K, c, ldc, splitk, partial, stream);

@@ -1,4 +1,4 @@
-// neighbors.cu -- neighbour search for the local-aggregation engine (sm_100a).
+// neighbors.cu -- neighbour search for the local-aggregation engine (sm_90a).
 //
 //   cl3d_ball_query    bit-exact replacement of the reference's masked_ordered_ball_query
 //                      (/root/reference/pytorch/ops/pt_custom_ops/_ext_src/src/masked_ordered_ball_query_gpu.cu:11-96)

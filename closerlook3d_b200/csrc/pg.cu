@@ -1,4 +1,4 @@
-// pg.cu -- PseudoGrid (KPConv-like) local aggregation, forward and backward, second generation (sm_100a).
+// pg.cu -- PseudoGrid (KPConv-like) local aggregation, forward and backward, second generation (sm_90a).
 //
 // Reference: /root/reference/pytorch/models/local_aggregation_operators.py:384-419
 //     h[k',m]  = clamp(1 - |dp_m - K_k'| / extent, min 0)                (linear; 'constant': 1)
@@ -9,16 +9,15 @@
 // ONE kernel template serves both directions: centre point p (query / support point), a list of neighbour rows
 // (features / upstream gradients).
 //
-// Why a second generation.  ncu on the first one (agg.cu; profiles/r2c_pg_v1_v2_summary.md): 1990 warp instructions
-// per query in the forward, of which 520 evaluate influences (16 scalar IEEE square roots per neighbour), 700 walk
-// the (neighbour, kernel point) pairs at 15 instructions per pair (bit scan + two address computations + three
-// 4-byte weight loads + three scalar FMAs), 125 reduce BatchNorm partials with shuffles; the backward kept 16
-// accumulators per channel (127 registers, 24 % of the warps resident).  Here:
-//   * a lane owns 4 CONSECUTIVE channels: one 16-byte load per neighbour row / weight row, packed fp32x2 arithmetic
-//     (fma.rn.f32x2 -> FFMA2 with a scalar-broadcast h operand);
+// Why a second generation.  The first one (agg.cu) spends most of its forward instructions on influences (16 scalar
+// IEEE square roots per neighbour) and on walking the (neighbour, kernel point) pairs at 15 instructions per pair (bit
+// scan + two address computations + three 4-byte weight loads + three scalar FMAs), plus shuffle reductions of the
+// BatchNorm partials; its backward keeps 16 accumulators per channel (127 registers).  Here:
+//   * a lane owns 4 CONSECUTIVE channels: one 16-byte load per neighbour row / weight row, arithmetic in channel
+//     pairs (FMAs with a scalar-broadcast h operand);
 //   * staging compiles, per neighbour with any non-zero influence, a list of (h, weight-row byte offset) entries
 //     -- 40 % of the neighbours have none and are dropped, the others ~3 of 15 -- so the pair loop is
-//     {8-byte entry load, 16-byte weight load, 2 FFMA2, branch}: 7 instructions instead of 15;
+//     {8-byte entry load, 16-byte weight load, 4 FFMA, branch}: 7 instructions instead of 15;
 //   * influences are evaluated straight-line and packed (two kernel points per instruction), the square root with
 //     the hardware approximation (2^-22 relative: h moves by < 3e-7, far inside the 1e-5 parity bar);
 //   * BatchNorm partial sums are accumulated per lane in registers and combined once per tile;
@@ -26,10 +25,8 @@
 //     accumulator addressed by the entry's offset: ~64 registers instead of 127.
 // One warp per centre point, 32 centre points per CTA tile; the backward is a persistent tile loop.
 //
-// Tried and measured on the same inputs, not shipped (profiles/RESULTS_r2.md): kernel weights and d/dWk accumulators
-// resident in registers with dense kernel-point quads (3x fewer shared-memory wavefronts, but 128 / 168 registers: 16 / 10
-// warps per SM cannot hide the load latencies -- 0.31 / 0.66 ms forward / backward at c3 against 0.27 / 0.48 here, and
-// 0.33 / 0.84 with a cross-point software pipeline that spilled).
+// Not shipped: kernel weights and d/dWk accumulators resident in registers with dense kernel-point quads (3x fewer
+// shared-memory wavefronts, but at 128 / 168 registers too few warps per SM stay resident to hide the load latencies).
 #include <stdlib.h>
 
 #include "agg_common.cuh"
@@ -39,7 +36,7 @@ namespace cl3d {
 constexpr int kPgWarps = 8;
 constexpr int kPgTile = 32;  // centre points per CTA tile
 // entries per staged neighbour + 1: rows of 17 float2 = 34 words put consecutive lanes' stores 2 banks apart (a
-// stride of 16 entries = 32 words sent every lane's store to the same banks: up to 26-way conflicts, r2e profile)
+// stride of 16 entries = 32 words sent every lane's store to the same banks: up to 26-way conflicts)
 constexpr int kEntStride = kMaxKP + 1;
 
 // dynamic shared memory of the PG kernels:
@@ -77,7 +74,7 @@ __host__ __device__ inline PgSmem pg_smem(int Cp, bool bwd) {
 
 // Coordinates of point r from a packed (n,3) array with two requests instead of three: the 12 bytes start 8-byte
 // aligned for even r (8 + 4) and end 8-byte aligned for odd r (4 + 8).  A scattered 4-byte load costs the L1 one
-// wavefront per distinct line and instruction, and these kernels are bound by exactly that (profiles/r2e).
+// wavefront per distinct line and instruction, and these kernels are bound by exactly that.
 __device__ __forceinline__ void load_xyz(const float* __restrict__ xyz, int r, float& x, float& y, float& z) {
   const float* p = xyz + (size_t)r * 3;
   if (r & 1) {
@@ -160,7 +157,7 @@ __device__ __forceinline__ void sts_f4(uint32_t addr, const float4& v) {
 // addresses of the warp's record / entry lists; `wk_a` / `pacc_a` = the lane's shared address inside the weight /
 // accumulator rows.  The next neighbour's row is requested before the current one is used.  The entry loop is kept
 // rolled on purpose: 8 instructions per entry; unrolled by the compiler it grew a 70-instruction remainder ladder
-// per neighbour (profiles/r2e).
+// per neighbour.
 template <bool BWD>
 __device__ __forceinline__ void pg_consume(const float* __restrict__ rows, uint32_t rec_a, uint32_t ent_a, uint32_t wk_a,
                                            uint32_t pacc_a, const float4& fown, bool owner, int n, float4& acc) {

@@ -1,7 +1,7 @@
 """CUDA-graph replay of one LocalAggregation training step (forward + backward).
 
 The hot path of a small cloud batch is ~40 short kernels; launched eagerly from Python the host cannot keep
-the GPU busy (measured on B200, BASELINE configs[1]: 1.3 ms of host time per step for 0.5 ms of kernels).
+the GPU busy: at the small BASELINE shapes the host time per step exceeds the kernel time.
 `GraphedStep` captures the whole step -- neighbour search, layout change, fused aggregation, BN, and the
 autograd backward -- once into a CUDA graph with static input / output buffers and replays it.  Nothing is
 cached between replays: every replay runs the full search and aggregation on whatever the static input

@@ -2,7 +2,7 @@
 (/root/reference/pytorch/models/local_aggregation_operators.py): the same five classes
     PosPool (:16)  AdaptiveWeight (:115)  PointWiseMLP (:227)  PseudoGrid (:319)  LocalAggregation (:429)
 with the same constructor / forward signatures and the same state-dict keys (checkpoints load unmodified),
-but each forward is ONE fused pass over libcl3d's sm_100a kernels instead of the reference's
+but each forward is ONE fused pass over libcl3d's sm_90a kernels instead of the reference's
 MaskedQueryAndGroup + ~10 elementwise torch ops over (B,C,M,K) tensors:
 
     neighbour search (grid hash, cached)  ->  fused gather + transform + reduce  ->  fused BN + ReLU

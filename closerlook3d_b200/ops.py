@@ -270,7 +270,7 @@ GEMM_AUTO, GEMM_FFMA, GEMM_TC3X = 0, 1, 2
 @_on_device
 def sgemm(a, sa_m, sa_k, b, sb_k, sb_n, M, N, K, out=None, ldc=None, splitk=1, algo=GEMM_AUTO):
     """out[m][n] = sum_k a[m*sa_m + k*sa_k] * b[k*sb_k + n*sb_n]  (element strides; fp32 accuracy: 3xTF32 on
-    the tcgen05 tensor cores, or the fp32 FMA kernel -- see cl3d.h)"""
+    the wgmma tensor cores, or the fp32 FMA kernel -- see cl3d.h)"""
     L = _lib.lib()
     dev = a.device
     ldc = N if ldc is None else ldc

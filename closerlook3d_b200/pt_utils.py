@@ -1,6 +1,6 @@
 """Drop-in replacement for the reference's `pt_utils` module
 (/root/reference/pytorch/ops/pt_custom_ops/pt_utils.py): same public names, constructor / forward
-signatures, return shapes and autograd behaviour, running on libcl3d's sm_100a kernels.
+signatures, return shapes and autograd behaviour, running on libcl3d's sm_90a kernels.
 
     reference name (pt_utils.py line)            here
     grouping_operation            (:64)          GroupingOperation.apply      -> cl3d_group_points[_grad]
@@ -105,7 +105,7 @@ overlap_enabled = True  # run the neighbour search on a side stream (fork/join),
 # Search the clouds of a batch in this many parts (clouds are independent).  The fused operators start the forward of
 # part 0 as soon as ITS search is done, so the issue-bound search of part 1 runs beside the L1-bound aggregation of
 # part 0 instead of in front of it.  1 = off.
-batch_parts = 1   # measured at c3 (profiles/RESULTS_r2.md): 2 parts 1.154 ms/step vs 1.107 -- half-batch kernels lose more to tail effects than the overlap wins
+batch_parts = 1   # splitting the batch trades overlap of search and aggregation for half-batch kernels with larger tail effects
 
 
 def _side_stream(device, priority=0):

@@ -1,5 +1,5 @@
 /*
- * cl3d.h -- C ABI of the Blackwell-native local-aggregation engine (libcl3d.so, sm_100a).
+ * cl3d.h -- C ABI of the H100-native local-aggregation engine (libcl3d.so, sm_90a).
  *
  * This is the drop-in boundary for the hot path of zeliu98/CloserLook3D (SURVEY.md section 8b).  It replaces
  * the reference's pybind module `pt_custom_ops._ext`
@@ -227,7 +227,7 @@ int cl3d_bn_relu_bwd(const float* grad_y, const float* x, const float* save_stat
 /* fp32 GEMM with element strides and optional split-K (gemm.cu, gemm_tc.cuh):
  *   C[m][n] = sum_k A[m*sa_m + k*sa_k] * B[k*sb_k + n*sb_n],  C row stride ldc.
  * splitk > 1 divides k among CTAs (fixed-order reduction); workspace = cl3d_sgemm_workspace_bytes.
- * algo: CL3D_GEMM_TC3X = tcgen05 tensor cores with the 3xTF32 operand split (fp32-level accuracy, the default
+ * algo: CL3D_GEMM_TC3X = wgmma tensor cores with the 3xTF32 operand split (fp32-level accuracy, the default
  * behind CL3D_GEMM_AUTO), CL3D_GEMM_FFMA = fp32 FMA pipe.  cl3d_sgemm == cl3d_sgemm_algo(..., CL3D_GEMM_AUTO). */
 #define CL3D_GEMM_AUTO 0
 #define CL3D_GEMM_FFMA 1

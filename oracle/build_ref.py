@@ -4,10 +4,10 @@
 TEST INFRASTRUCTURE ONLY.  Nothing in the product path (closerlook3d_b200/) imports this.
 
 The reference's native ops (pytorch/ops/pt_custom_ops/_ext_src, 4 .cu + 5 .cpp files) are compiled
-*from where they lie* under /root/reference with a hand-written nvcc/g++ recipe (the reference's own
-setup.py is not run), for sm_100 (plain, as the reference would be built by TORCH_CUDA_ARCH_LIST=10.0),
-with the reference's own flags (-O2, no fast-math).  Outputs go only into oracle/_ref/ (git-ignored,
-not gpurun-ignored, so the .so travels to the GPU box).  On the GPU box the result is used as
+*from where they lie* in a checkout of the reference (CL3D_REFERENCE, default /root/reference) with a
+hand-written nvcc/g++ recipe (the reference's own setup.py is not run), for sm_90 (plain, as the reference
+would be built by TORCH_CUDA_ARCH_LIST=9.0), with the reference's own flags (-O2, no fast-math).  Outputs go
+only into oracle/_ref/ (git-ignored).  Where it is built, the result is used as
 
   * the GPU-side pin for the C restatement in oracle/cl3d_oracle.c (bit-exact idx / idx_mask / sub_xyz), and
   * the "reference GPU path" timing in bench.py (extra, informational).
@@ -21,7 +21,7 @@ import sysconfig
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_SRC = "/root/reference/pytorch/ops/pt_custom_ops/_ext_src"
+REF_SRC = os.path.join(os.environ.get("CL3D_REFERENCE", "/root/reference"), "pytorch/ops/pt_custom_ops/_ext_src")
 OUT_DIR = os.path.join(HERE, "_ref", "pt_custom_ops")
 SO_NAME = "_ext" + sysconfig.get_config_var("EXT_SUFFIX")
 
@@ -36,8 +36,8 @@ def built_path():
 
 
 def build(force=False, verbose=True):
-    """Compile the reference extension.  Returns the .so path, or None when /root/reference is absent
-    (GPU box: the prebuilt file is used)."""
+    """Compile the reference extension.  Returns the .so path, or None when the reference checkout is absent
+    (a previously built file is used if there is one)."""
     if not ref_available():
         return built_path()
     if built_path() and not force:
@@ -60,7 +60,7 @@ def build(force=False, verbose=True):
         obj = os.path.join(obj_dir, s + ".o")
         objs.append(obj)
         if s.endswith(".cu"):
-            cmd = ["nvcc", "-c", src, "-o", obj, "-O2", "-gencode", "arch=compute_100,code=sm_100",
+            cmd = ["nvcc", "-c", src, "-o", obj, "-O2", "-gencode", "arch=compute_90,code=sm_90",
                    "--compiler-options", "-fPIC", "--expt-relaxed-constexpr"] + common + inc_flags
         elif s.endswith(".cpp"):
             cmd = ["g++", "-c", src, "-o", obj, "-O2", "-fPIC"] + common + inc_flags
@@ -91,7 +91,7 @@ def load():
     """Import the compiled reference extension as module `pt_custom_ops._ext` (needs a GPU to be useful)."""
     so = built_path()
     if so is None:
-        raise ImportError("oracle/_ref is not built (run oracle/build_ref.py where /root/reference exists)")
+        raise ImportError("oracle/_ref is not built (run oracle/build_ref.py where the reference checkout exists)")
     import importlib.util
     import torch  # noqa: F401  (must be loaded first: the .so links against libtorch)
     spec = importlib.util.spec_from_file_location("_ext", so)

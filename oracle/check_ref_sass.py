@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Check (container only) that the sm_100 SASS nvcc emits for the reference's distance expression is
+"""Check (container only) that the sm_90 SASS nvcc emits for the reference's distance expression is
     FADD dy ; FADD dx ; FMUL t=dy*dy ; FADD dz ; FFMA t=dx*dx+t ; FFMA t=dz*dz+t
 i.e. d2 = fma(dz,dz, fma(dx,dx, dy*dy)) with d = query - support, which is what oracle/cl3d_oracle.c (ref_d2)
 and closerlook3d_b200/csrc/common.cuh (ref_d2) spell out.  Needs oracle/_ref/obj (run oracle/build_ref.py).

@@ -1,9 +1,9 @@
-"""oracle/ref_loader.py -- import the UNMODIFIED reference python hot path on CPU (container only).
+"""oracle/ref_loader.py -- import the UNMODIFIED reference python hot path on CPU.
 
-TEST INFRASTRUCTURE ONLY.  Used by oracle/make_golden.py and the `-m "not gpu"` validation tests that
-run where /root/reference exists; never on the GPU box, never by the product.
+TEST INFRASTRUCTURE ONLY.  Used by oracle/make_golden.py and oracle/make_ref_vectors.py where a reference checkout
+exists (CL3D_REFERENCE, default /root/reference); never by the tests or the product.
 
-Three shims make `/root/reference/pytorch/{models,ops/pt_custom_ops/pt_utils.py,utils/config.py}` import
+Three shims make `<reference>/pytorch/{models,ops/pt_custom_ops/pt_utils.py,utils/config.py}` import
 as they are (SURVEY.md section 8c):
   1. sys.modules['pt_custom_ops._ext'] = oracle.ext   (the reference's native ops are CUDA-only)
   2. an `easydict.EasyDict` stand-in                  (package not installed here)
@@ -16,7 +16,7 @@ import sys
 import tempfile
 import types
 
-REF_ROOT = "/root/reference/pytorch"
+REF_ROOT = os.path.join(os.environ.get("CL3D_REFERENCE", "/root/reference"), "pytorch")
 
 
 def available():
@@ -53,7 +53,7 @@ def load(ext_module=None):
     if "ns" in _loaded:
         return _loaded["ns"]
     if not available():
-        raise ImportError("/root/reference is not present (GPU box?) -- use tests/golden fixtures instead")
+        raise ImportError(f"{REF_ROOT} is not present -- the tests use the tests/golden fixtures instead")
     from . import ext as oracle_ext
     ext_module = ext_module or oracle_ext
     pkg = types.ModuleType("pt_custom_ops")

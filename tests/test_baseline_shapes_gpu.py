@@ -3,7 +3,7 @@ backward, against the reference's own GPU path = oracle/la_oracle.py on top of t
 extension (oracle/_ref), TF32 off, same seeded inputs.
 
 Why these sizes matter: every gather-form backward is a persistent kernel (grid = min(tiles, 4 x SMs) with a
-`tile += gridDim.x` loop and state carried across tiles); only B * ceil(N/32) > 4 * 148 = 592 tiles exercises
+`tile += gridDim.x` loop and state carried across tiles); only B * ceil(N/32) > 4 * 132 = 528 tiles (H100) exercises
 that loop.  c2: 1024 tiles, c3: 3752, c4: 1252, c5 (2 of the 8 clouds per GPU): 2500.
 
 Bars (BASELINE.json north_star): outputs and feature gradients <= 1e-5 of max; parameter gradients <= 5e-5

@@ -1,6 +1,7 @@
 """CPU tests (-m "not gpu"): the oracle is pinned against
   (1) the golden fixtures made by the UNMODIFIED reference python modules (tests/golden, bit-exact),
-  (2) the live reference modules where /root/reference exists (container),
+  (2) outputs and feature gradients the unmodified reference modules computed on seeded clouds
+      (tests/golden/ref_la_*.pt, recorded by oracle/make_ref_vectors.py),
   (3) an independent pure-python restatement of the ball-query rule on tiny inputs + structural properties.
 """
 import copy
@@ -12,7 +13,7 @@ import pytest
 import torch
 
 from closerlook3d_b200 import synth
-from closerlook3d_b200.config import la_config
+from closerlook3d_b200.config import AttrDict, la_config
 
 GOLD = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "la_*.pt")))
 
@@ -32,19 +33,18 @@ def test_oracle_reproduces_reference_golden(oracle_ext, path):
     (out * g["grad_out"]).sum().backward()
     assert torch.equal(out.detach(), g["out"])                       # same torch ops in the same order
     assert torch.equal(f.grad, g["grad_features"])
+    # parameter gradients are reductions inside torch's CPU convolution / matmul kernels, whose summation order
+    # depends on the host's instruction set: equal up to fp32 reordering, not bit for bit, across machines
     for k, v in orc.grads().items():
-        assert torch.equal(v, g["grad_params"]["local_aggregation_operator." + k]), k
+        want = g["grad_params"]["local_aggregation_operator." + k]
+        assert float((v - want).abs().max()) <= 1e-6 * max(1.0, float(want.abs().max())), k
     for k, v in orc.st.items():
         if k.endswith(("running_mean", "running_var", "num_batches_tracked")):
             assert torch.equal(v, g["state_dict_after"]["local_aggregation_operator." + k]), k
 
 
-def _ref_available():
-    return os.path.isdir("/root/reference/pytorch/models")
-
-
-@pytest.mark.skipif(not _ref_available(), reason="/root/reference not present (GPU box)")
-@pytest.mark.parametrize("la_type,over", [
+LA_SHAPE = (2, 300, 10, 24)   # B, N, K, C
+LIVE_CASES = [
     ("pospool", dict(pospool=dict(position_embedding="xyz", reduction="avg"))),
     ("pospool", dict(pospool=dict(position_embedding="sin_cos", reduction="sum"))),
     ("adaptive_weight", dict(adaptive_weight=dict(num_mlps=2, shared_channels=2, reduction="avg"))),
@@ -54,25 +54,33 @@ def _ref_available():
     ("pospool", dict(pospool=dict(position_embedding="xyz", reduction="max"))),
     ("pospool", dict(pospool=dict(position_embedding="sin_cos", reduction="max"))),
     ("adaptive_weight", dict(adaptive_weight=dict(num_mlps=1, shared_channels=1, reduction="max"))),
-])
+]
+
+
+def live_case_id(la_type, over):
+    v = over.get(la_type, {})
+    return "_".join([la_type] + [f"{k}-{v[k]}" for k in sorted(v)])
+
+
+def _attr(d):
+    return AttrDict({k: _attr(v) if isinstance(v, dict) else v for k, v in d.items()})
+
+
+@pytest.mark.parametrize("la_type,over", LIVE_CASES)
 def test_oracle_matches_live_reference(oracle_ext, la_type, over):
-    from oracle import la_oracle, ref_loader
-    ns = ref_loader.load()
-    torch.manual_seed(1)
-    B, N, K, C = 2, 300, 10, 24
-    cfg = ref_loader.make_config(la_type, **over)
+    """the oracle == what the unmodified reference modules computed on the same seeded cloud, bit for bit"""
+    from oracle import la_oracle
+    g = torch.load(os.path.join(os.path.dirname(__file__), "golden", f"ref_la_{live_case_id(la_type, over)}.pt"),
+                   weights_only=False)
+    B, N, K, C = LA_SHAPE
+    cfg = _attr(g["cfg"])
     r = synth.ball_radius(N, K)
-    ref = ns.lao.LocalAggregation(C, C, r, K, cfg)
-    sd = copy.deepcopy(ref.state_dict())
     d = synth.make_cloud_batch(B, N, C, 9)
-    f1 = d["features"].clone().requires_grad_(True)
     f2 = d["features"].clone().requires_grad_(True)
-    o1 = ref(d["xyz"], d["xyz"], d["mask"], d["mask"], f1)
-    orc = la_oracle.OracleLocalAggregation(oracle_ext, la_type, C, C, r, K, cfg, sd)
+    orc = la_oracle.OracleLocalAggregation(oracle_ext, la_type, C, C, r, K, cfg, g["state_dict"])
     o2 = orc(d["xyz"], d["xyz"], d["mask"], d["mask"], f2)
-    o1.sum().backward()
     o2.sum().backward()
-    assert torch.equal(o1, o2) and torch.equal(f1.grad, f2.grad)
+    assert torch.equal(g["out"], o2) and torch.equal(g["grad_features"], f2.grad)
 
 
 def _py_ball_query(q, s, qm, sm, radius, K):

@@ -1,5 +1,5 @@
 """GPU pins against the reference's OWN CUDA extension (oracle/_ref: the reference sources compiled unmodified
-for sm_100 by oracle/build_ref.py):
+for sm_90 by oracle/build_ref.py):
   * the C restatement (oracle/cl3d_oracle.c) equals the reference kernels bit for bit  -> the oracle is pinned;
   * libcl3d equals the reference kernels bit for bit at the FULL BASELINE sizes, where the CPU oracle is slow.
 Skipped when oracle/_ref has not been built (it is built in the container and travels with the snapshot)."""
