@@ -353,11 +353,15 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_bwd_dense_kernel(const Pw
 //   grad_A[j_0(q)] += da'      one 16-byte vector reduction (red.global.add.v4.f32) per (query, 4 channels)
 //   grad_T[idx[q][k*]] += sgn*sc*dz  at the arg-max slot of each channel (scalar red.add, non-zero only)
 //   d/dWp -= da' (x) q/r      per-CTA partial (gridDim.x, 3, Cout), reduced afterwards in a fixed order
-constexpr int kPWQPT = 8;  // queries per thread
+// Layers wider than 4 * kPWQGroups channels split their channel groups over blockIdx.y (one slice per CTA).
+constexpr int kPWQPT = 8;        // queries per thread
+constexpr int kPWQGroups = 256;  // channel groups of 4 per CTA slice (= the block size when ny = 1)
 __global__ void __launch_bounds__(256) pwmlp_bwd_query_kernel(const PwArgs a, long long nqueries /* B*M */) {
   extern __shared__ float s_dw[];  // [ny][3][Cop]
-  const int nx = a.Cop >> 2, ny = blockDim.x / nx;
-  const int x = threadIdx.x % nx, y = threadIdx.x / nx;
+  const int ngroups = a.Cop >> 2;
+  const int nx = ngroups < kPWQGroups ? ngroups : kPWQGroups, ny = blockDim.x / nx;
+  const int x = blockIdx.y * nx + threadIdx.x % nx, y = threadIdx.x / nx;
+  const bool active = x < ngroups;  // the last slice of a wide layer may be narrower than nx
   const int c4 = x * 4;
   float c1[4], c2[4], mean[4], sg[4], dw[3][4];
 #pragma unroll
@@ -378,7 +382,7 @@ __global__ void __launch_bounds__(256) pwmlp_bwd_query_kernel(const PwArgs a, lo
 #pragma unroll 2
     for (int it = 0; it < kPWQPT; ++it) {
       const long long gq = qbase + (long long)it * ny + y;  // b*M + q
-      if (gq >= nqueries) break;
+      if (gq >= nqueries || !active) break;
       const long long b = gq / a.M;
       const size_t o = (size_t)gq * a.Cop + c4;
       const float4 ap = *reinterpret_cast<const float4*>(a.aq + o);
@@ -408,17 +412,20 @@ __global__ void __launch_bounds__(256) pwmlp_bwd_query_kernel(const PwArgs a, lo
       asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(pa), "f"(da[0]), "f"(da[1]), "f"(da[2]), "f"(da[3])
                    : "memory");
     }
+    if (active)
 #pragma unroll
-    for (int s3 = 0; s3 < 3; ++s3)
+      for (int s3 = 0; s3 < 3; ++s3)
 #pragma unroll
-      for (int t = 0; t < 4; ++t) s_dw[((size_t)y * 3 + s3) * a.Cop + c4 + t] = dw[s3][t];
+        for (int t = 0; t < 4; ++t) s_dw[((size_t)y * 3 + s3) * a.Cop + c4 + t] = dw[s3][t];
   }
   __syncthreads();
-  for (int e = threadIdx.x; e < 3 * a.Cout; e += blockDim.x) {
-    const int s3 = e / a.Cout, c = e % a.Cout;
+  // this CTA's channels [cs0, cs0 + w)
+  const int cs0 = blockIdx.y * nx * 4, w = min(nx * 4, a.Cout - cs0);
+  for (int e = threadIdx.x; e < 3 * w; e += blockDim.x) {
+    const int s3 = e / w, c = cs0 + e % w;
     float t = 0.f;
     for (int yy = 0; yy < ny; ++yy) t += s_dw[((size_t)yy * 3 + s3) * a.Cop + c];
-    a.partial[(size_t)blockIdx.x * 3 * a.Cout + e] = t;
+    a.partial[((size_t)blockIdx.x * 3 + s3) * a.Cout + c] = t;
   }
 }
 
@@ -519,7 +526,7 @@ static int pw_dense_grid(int ntiles_n) {
   return gx > ntiles_n ? ntiles_n : gx;
 }
 static int pw_query_grid(int B, int M, int Cop) {
-  const int ny = 256 / (Cop / 4) > 0 ? 256 / (Cop / 4) : 1;
+  const int ny = 256 / (Cop / 4 < kPWQGroups ? Cop / 4 : kPWQGroups);  // queries per CTA row (pwmlp_bwd_query_kernel)
   return (int)(((long long)B * M + (long long)ny * kPWQPT - 1) / ((long long)ny * kPWQPT));
 }
 
@@ -697,9 +704,9 @@ extern "C" int cl3d_pwmlp_bwd(const float* grad_out, const float* out, const flo
     }
     if (rc) return rc;
   }
-  CL3D_REQUIRE(Cop / 4 <= 256, "cl3d_pwmlp_bwd: Cout > 1024 unsupported");
-  const int ny = 256 / (Cop / 4);
-  pwmlp_bwd_query_kernel<<<gqy, ny * (Cop / 4), (size_t)ny * 3 * Cop * sizeof(float), side>>>(a, (long long)B * M);
+  const int nx = Cop / 4 < kPWQGroups ? Cop / 4 : kPWQGroups, ny = 256 / nx;
+  pwmlp_bwd_query_kernel<<<dim3(gqy, ceil_div(Cop / 4, nx)), ny * nx, (size_t)ny * 3 * Cop * sizeof(float), side>>>(
+      a, (long long)B * M);
   CL3D_LAUNCHED(1);
   rc = check_launch("pwmlp_bwd_query_kernel");
   if (rc) return rc;

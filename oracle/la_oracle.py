@@ -59,7 +59,8 @@ DIM_MAT_FN = None
 # Checker-side diagnostics: when this is a dict, pointwise_mlp() leaves its pre-max activations (B,C,M,K) and the
 # neighbour indices (B,M,K) in it, so that a parity test can find the (query, channel) positions whose two best
 # DISTINCT neighbours are closer than the comparison tolerance -- there the arg-max, and with it the gradient
-# routing, is decided by rounding (see argmax_is_decided()).
+# routing, is decided by rounding (see argmax_is_decided()).  The max reductions of the other families leave their
+# pre-max products ("premax"), and every family its output before the final ReLU ("pre_relu").
 KEEP = None
 
 
@@ -94,6 +95,8 @@ def query_and_group(ext, query_xyz, support_xyz, query_mask, support_mask, featu
             grouped_xyz = grouped_xyz * inv                                   # what the CUDA kernel computes
         else:
             grouped_xyz = grouped_xyz / radius                                # :128-129 true division by float(radius)
+    if features is not None:   # float64 run: dp is formed in fp32 like the reference, then joins the features' dtype
+        grouped_xyz = grouped_xyz.to(features.dtype)
     grouped_features = group(features, idx) if features is not None else None
     if KEEP is not None:
         KEEP["idx"] = idx.long()
@@ -162,8 +165,12 @@ def _out_block(out, st, cfg_out_conv, cin, cout, momentum, training):
     """out_conv (Conv1d 1x1 no bias + BN1d + ReLU) or out_transform (BN1d + ReLU): :37-45,107-110"""
     if cfg_out_conv or cin != cout:
         out = F.conv1d(out, st["out_conv.0.weight"])
-        return F.relu(_bn(out, st, "out_conv.1", momentum, training))
-    return F.relu(_bn(out, st, "out_transform.0", momentum, training))
+        y = _bn(out, st, "out_conv.1", momentum, training)
+    else:
+        y = _bn(out, st, "out_transform.0", momentum, training)
+    if KEEP is not None:
+        KEEP["pre_relu"] = y.detach()
+    return F.relu(y)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -180,7 +187,9 @@ def pospool(ext, st, cfg, cin, cout, radius, nsample, q_xyz, s_xyz, q_mask, s_ma
         fd = C // 6
         rng = torch.arange(fd, dtype=torch.float32, device=q_xyz.device)
         dim_mat = torch.pow(1.0 * 1000, (1.0 / fd) * rng) if DIM_MAT_FN is None else DIM_MAT_FN(fd).to(rng.device)
-        div = torch.div((100 * dp).unsqueeze(-1), dim_mat)                   # (B,3,M,K,fd)
+        # the argument fl32(fl32(100 dp) / dim) is part of the reference's function: it is formed in fp32 even in a
+        # float64 run (one ulp of it moves sin by ~1e-5), only sin / cos are then taken in the features' dtype
+        div = torch.div((100 * dp.float()).unsqueeze(-1), dim_mat).to(gf.dtype)   # (B,3,M,K,fd)
         emb = torch.cat([torch.sin(div), torch.cos(div)], -1)                # (B,3,M,K,2fd)
         emb = emb.permute(0, 1, 4, 2, 3).contiguous().view(B, C, M, nsample)
         agg = gf * emb
@@ -216,9 +225,12 @@ def pointwise_mlp(ext, st, cfg, cin, cout, radius, nsample, q_xyz, s_xyz, q_mask
     x = torch.cat([dp, center, gf - center], 1)
     for i in range(pw.num_mlps):                                              # :252-272 conv + BN2d + ReLU
         x = F.conv2d(x, st[f"mlps.conv{i}.0.weight"])
-        x = F.relu(_bn(x, st, f"mlps.conv{i}.1", cfg.bn_momentum, training))
+        y = _bn(x, st, f"mlps.conv{i}.1", cfg.bn_momentum, training)
+        x = F.relu(y)
     if KEEP is not None:
         KEEP["pwmlp_premax"], KEEP["idx"] = x.detach(), idx.long()
+        if pw.reduction == "max":   # max_k relu(y) = relu(max_k y): the output's value before the ReLU
+            KEEP["pre_relu"] = y.detach().max(dim=-1)[0]
     return _reduce(x, idx_mask, q_mask, pw.reduction)                         # no out_transform (:297-316)
 
 
@@ -258,18 +270,23 @@ class OracleLocalAggregation:
 
     state: dict key -> tensor, keys as in the reference module's state_dict() (with or without the
     'local_aggregation_operator.' prefix).  Float tensors that the reference registers as Parameters get
-    requires_grad=True so .grads() mirrors the reference's parameter gradients."""
+    requires_grad=True so .grads() mirrors the reference's parameter gradients.
+    dtype: cast every floating state tensor (parameters, BatchNorm state, kernel points) to it, e.g. torch.float64
+    with oracle.f64_ext as `ext` for a high-precision reference; None keeps the state's own dtype."""
 
     PREFIX = "local_aggregation_operator."
     _BUFFERS = ("running_mean", "running_var", "num_batches_tracked", "K_points")
 
-    def __init__(self, ext, la_type, in_channels, out_channels, radius, nsample, cfg, state, device="cpu"):
+    def __init__(self, ext, la_type, in_channels, out_channels, radius, nsample, cfg, state, device="cpu",
+                 dtype=None):
         self.ext, self.la_type = ext, la_type
         self.cin, self.cout, self.radius, self.nsample, self.cfg = in_channels, out_channels, radius, nsample, cfg
         self.st = {}
         for k, v in state.items():
             k = k[len(self.PREFIX):] if k.startswith(self.PREFIX) else k
             v = v.detach().clone().to(device)
+            if dtype is not None and v.is_floating_point():
+                v = v.to(dtype)
             if v.is_floating_point() and not k.endswith(self._BUFFERS):
                 v.requires_grad_(True)
             self.st[k] = v
