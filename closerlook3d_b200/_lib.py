@@ -61,7 +61,23 @@ SIGNATURES = {
     "cl3d_pwmlp_fwd_out": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "cl3d_pwmlp_bwd_scratch_floats": (_sz, [_i, _i, _i, _i]),
     "cl3d_pwmlp_bwd": (_i, [_vp] * 16 + [_i, _i, _i, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "cl3d_mhead_save_floats": (_sz, [_i, _i]),
+    "cl3d_mhead_fwd_workspace_bytes": (_sz, [_vp, _i, _i]),
+    "cl3d_mhead_bwd_workspace_bytes": (_sz, [_vp, _i, _i]),
+    "cl3d_mhead_fwd": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _f, _f, _i, _vp, _vp, _vp, _sz, _vp]),
+    "cl3d_mhead_bwd": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
+
+MHEAD_MAX_HEADS = 32       # CL3D_MHEAD_MAX_HEADS
+MHEAD_MAX_PARTS = 64       # CL3D_MHEAD_MAX_PARTS
+MHEAD_MAX_CHANNELS = 128   # CL3D_MHEAD_MAX_CHANNELS (padded)
+
+
+class MHeadDesc(ctypes.Structure):
+    """struct cl3d_mhead_desc (passed by host pointer, copied into the kernels' arguments)"""
+    _fields_ = [("S", _i), ("C", _i), ("num_parts", _i * MHEAD_MAX_HEADS),
+                ("running_mean", _vp * MHEAD_MAX_HEADS), ("running_var", _vp * MHEAD_MAX_HEADS),
+                ("num_batches_tracked", _vp * MHEAD_MAX_HEADS), ("grad_logits", _vp * MHEAD_MAX_HEADS)]
 
 
 class _Profiler:
@@ -111,7 +127,8 @@ def _wrap(name, fn):
 
 _UNTIMED = {"cl3d_version", "cl3d_last_error", "cl3d_padded_channels", "cl3d_sm_count", "cl3d_launch_count",
             "cl3d_ball_query_workspace_bytes", "cl3d_ball_query_csr_workspace_bytes", "cl3d_csr_workspace_bytes", "cl3d_grid_subsample_workspace_bytes",
-            "cl3d_agg_num_tiles", "cl3d_agg_bwd_num_blocks", "cl3d_agg_num_params", "cl3d_sgemm_workspace_bytes", "cl3d_pwmlp_bwd_scratch_floats"}
+            "cl3d_agg_num_tiles", "cl3d_agg_bwd_num_blocks", "cl3d_agg_num_params", "cl3d_sgemm_workspace_bytes", "cl3d_pwmlp_bwd_scratch_floats",
+            "cl3d_mhead_save_floats", "cl3d_mhead_fwd_workspace_bytes", "cl3d_mhead_bwd_workspace_bytes"}
 
 
 def lib():

@@ -7,7 +7,10 @@ package's operators.
     models/backbones/resnet.py:71-188   ResNet                     ResNet  (stages built in a loop)
     models/heads/classifier.py:6-52     ClassifierResNet           ClassifierResNet
     models/heads/segmentation_head.py:15-94  SceneSegHeadResNet    SceneSegHeadResNet
-    models/build.py:9-33,36-122         build_* / *Model           build_classification / build_scene_segmentation
+    models/heads/segmentation_head.py:97-149 MultiPartSegHeadResNet MultiPartSegHeadResNet (heads: partseg.py, fused)
+    models/build.py:9-33,36-122         build_* / *Model           build_classification / build_scene_segmentation /
+                                                                   build_multi_part_segmentation
+    losses/multi_shape_cross_entropy.py MultiShapeCrossEntropy     multi_shape_cross_entropy
 
 The reference's own `models/` also run on this package with zero edits through `shim.install()`; this module exists so
 that the whole-model path is available (and testable on the GPU box) without the reference tree.  The 1x1 convolutions
@@ -20,6 +23,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .local_aggregation_operators import LocalAggregation
+from .partseg import multi_shape_heads_forward
 from .pt_utils import MaskedMaxPool, MaskedUpsample
 
 
@@ -154,6 +158,35 @@ class SceneSegHeadResNet(nn.Module):
         return self.head(features)
 
 
+class MultiPartSegHeadResNet(nn.Module):
+    """the scene-segmentation decoder followed by one head per shape category, Conv1d(C,C) + BN + ReLU +
+    Conv1d(C, num_parts[s]) with C = width/2, all run over every point (segmentation_head.py:97-149).  The heads run
+    fused (partseg.py); forward returns the reference's list of S logits tensors (B, num_parts[s], N)."""
+
+    def __init__(self, num_classes, width, base_radius, nsamples, num_parts):
+        super().__init__()
+        self.num_classes, self.base_radius, self.nsamples, self.num_parts = num_classes, base_radius, nsamples, num_parts
+        cins = [24 * width, 8 * width, 4 * width, 2 * width]
+        couts = [4 * width, 2 * width, width, width // 2]
+        for i in range(4):
+            setattr(self, f"up{i}", MaskedUpsample(radius=(8 >> i) * base_radius, nsample=nsamples[3 - i], mode="nearest"))
+        for i in range(4):
+            setattr(self, f"up_conv{i}", _conv_bn(cins[i], couts[i], 0.1, relu=True))
+        self.multi_shape_heads = nn.ModuleList()
+        for i in range(num_classes):
+            self.multi_shape_heads.append(nn.Sequential(*list(_conv_bn(width // 2, width // 2, 0.1, relu=True)),
+                                                        nn.Conv1d(width // 2, num_parts[i], kernel_size=1, bias=True)))
+
+    def forward(self, end_points):
+        features = end_points["res5_features"]
+        for i in range(4):
+            fine, coarse = f"res{4 - i}", f"res{5 - i}"
+            features = getattr(self, f"up{i}")(end_points[fine + "_xyz"], end_points[coarse + "_xyz"],
+                                               end_points[fine + "_mask"], end_points[coarse + "_mask"], features)
+            features = getattr(self, f"up_conv{i}")(torch.cat([features, end_points[fine + "_features"]], 1))
+        return multi_shape_heads_forward(self.multi_shape_heads, features)
+
+
 class _Model(nn.Module):
     def _make_backbone(self, config):
         if config.backbone != "resnet":
@@ -198,6 +231,21 @@ class SceneSegmentationModel(_Model):
         return self.segmentation_head(self.backbone(xyz, mask, features))
 
 
+class MultiPartSegmentationModel(_Model):
+    """backbone + `segmentation_head` (build.py:66-90): forward -> list of S logits (B, num_parts[s], N)"""
+
+    def __init__(self, config):
+        super().__init__()
+        self.backbone = self._make_backbone(config)
+        if config.head != "resnet_part_seg":
+            raise NotImplementedError(f"Head {config.head} not implemented in Multi-Part Segmentation Model")
+        self.segmentation_head = MultiPartSegHeadResNet(config.num_classes, config.width, config.radius,
+                                                        config.nsamples, config.num_parts)
+
+    def forward(self, xyz, mask, features):
+        return self.segmentation_head(self.backbone(xyz, mask, features))
+
+
 def label_smoothing_cross_entropy(pred, target, smoothing_ratio=0.2):
     """the classification criterion (losses/label_smoothing_cross_entropy.py:6-21)"""
     n = pred.size(1)
@@ -211,6 +259,21 @@ def masked_cross_entropy(logit, target, mask):
     return loss.sum() / mask.sum()
 
 
+def multi_shape_cross_entropy(logits_all_shapes, points_labels, shape_labels):
+    """the part-segmentation criterion (losses/multi_shape_cross_entropy.py:6-23): per sample, the mean cross entropy
+    of its own shape's logits over all N points (unmasked), plus 0 * the sum of every other shape's logits, over B.
+    Written per head with a sample selector instead of a Python loop over samples: same value and gradients, no
+    host synchronisation."""
+    B = shape_labels.shape[0]
+    loss = 0.0
+    for s, logits in enumerate(logits_all_shapes):
+        sel = shape_labels == s
+        target = torch.where(sel[:, None], points_labels, torch.zeros_like(points_labels))
+        ce = F.cross_entropy(logits, target, reduction="none").mean(1)
+        loss = loss + torch.where(sel, ce, 0.0 * logits.sum((1, 2))).sum()
+    return loss / B
+
+
 def build_classification(config):
     return ClassificationModel(config), label_smoothing_cross_entropy
 
@@ -219,9 +282,29 @@ def build_scene_segmentation(config):
     return SceneSegmentationModel(config), masked_cross_entropy
 
 
-def model_config(task="classification", local_aggregation_type="pospool", **overrides):
+def build_multi_part_segmentation(config):
+    return MultiPartSegmentationModel(config), multi_shape_cross_entropy
+
+
+# The shipped part-segmentation settings (cfgs/partnet/*.yaml, cfgs/shapenetpart/*.yaml): the same for every family
+# except ShapeNetPart's PointWiseMLP batch (12).
+PART_DATASETS = {
+    "partnet": dict(datasets="partnet", num_classes=17,
+                    num_parts=[15, 9, 39, 11, 7, 4, 5, 10, 12, 10, 41, 6, 7, 24, 51, 11, 6], input_features_dim=3,
+                    batch_size=8, num_points=10000, radius=0.05, sampleDl=0.02, nsamples=[23, 38, 42, 40, 36],
+                    npoints=[5120, 1024, 384, 64], bn_momentum=0.01),
+    "shapenetpart": dict(datasets="shapenetpart", num_classes=16,
+                         num_parts=[4, 2, 2, 4, 4, 3, 3, 2, 4, 2, 6, 2, 3, 3, 3, 3], input_features_dim=3,
+                         batch_size=16, num_points=2048, radius=0.05, sampleDl=0.02, nsamples=[11, 25, 37, 36, 33],
+                         npoints=[1280, 768, 192, 64], bn_momentum=0.1),
+}
+
+
+def model_config(task="classification", local_aggregation_type="pospool", dataset=None, **overrides):
     """A stand-alone config with the reference's model defaults (utils/config.py:20-33) and the shipped cfgs' stage
-    settings: cfgs/modelnet/*.yaml for classification, cfgs/s3dis/*.yaml for scene segmentation."""
+    settings: cfgs/modelnet/*.yaml for classification, cfgs/s3dis/*.yaml for scene segmentation, and for
+    multi_part_segmentation cfgs/partnet/*.yaml (dataset=None or "partnet") or cfgs/shapenetpart/*.yaml
+    (dataset="shapenetpart").  N of PartNet (no num_points key in its yaml) is the dataset's 10000 points."""
     from .config import la_config
     c = la_config(local_aggregation_type, **{k: v for k, v in overrides.items() if isinstance(v, dict)})
     c.backbone, c.width, c.depth, c.bottleneck_ratio = "resnet", 144, 2, 2
@@ -231,6 +314,12 @@ def model_config(task="classification", local_aggregation_type="pospool", **over
     elif task == "scene_segmentation":
         c.update(head="resnet_scene_seg", num_classes=13, input_features_dim=4, radius=0.1, sampleDl=0.04,
                  nsamples=[26, 31, 38, 41, 39], npoints=[4096, 1152, 304, 88], num_points=15000)
+    elif task == "multi_part_segmentation":
+        d = dict(PART_DATASETS[dataset or "partnet"])
+        d["num_parts"], d["nsamples"], d["npoints"] = list(d["num_parts"]), list(d["nsamples"]), list(d["npoints"])
+        if d["datasets"] == "shapenetpart" and local_aggregation_type == "pointwisemlp":
+            d["batch_size"] = 12
+        c.update(head="resnet_part_seg", **d)
     else:
         raise NotImplementedError(task)
     for k, v in overrides.items():

@@ -4,7 +4,8 @@ The reference reaches the hot path through two bare module names put on sys.path
 (`from pt_utils import MaskedQueryAndGroup`, models/local_aggregation_operators.py:13; `from pt_utils import
 MaskedMaxPool`, models/backbones/resnet.py:11; `MaskedUpsample`, models/heads/segmentation_head.py:12) and
 through `from ..local_aggregation_operators import LocalAggregation` (resnet.py:3).  `install()` pre-seeds
-sys.modules so that those imports resolve to this package's drop-in modules.  It also provides the two small
+sys.modules so that those imports resolve to this package's drop-in modules, and re-binds the reference's
+MultiPartSegHeadResNet to this package's (same module tree, heads fused).  It also provides the two small
 compatibility shims the reference needs on a current stack (easydict not installed; yaml.load without Loader).
 """
 import importlib
@@ -56,6 +57,16 @@ def install(reference_pytorch_root=None):
                     for attr in ("LocalAggregation", "PosPool", "AdaptiveWeight", "PointWiseMLP", "PseudoGrid"):
                         if hasattr(mod, attr) and getattr(mod, attr) is not getattr(lao, attr):
                             setattr(mod, attr, getattr(lao, attr))
+            # the part-segmentation head runs its S shape heads fused: models/build.py binds the class by name
+            # (`from .heads import MultiPartSegHeadResNet`), so every module that holds it is re-bound
+            from .backbone import MultiPartSegHeadResNet
+            for name in ("models.heads.segmentation_head", "models.heads", "models.build"):
+                try:
+                    mod = importlib.import_module(name)
+                except ImportError:
+                    continue
+                if hasattr(mod, "MultiPartSegHeadResNet"):
+                    mod.MultiPartSegHeadResNet = MultiPartSegHeadResNet
 
 
 def reference_config(yaml_path):

@@ -46,3 +46,14 @@ def baseline_inputs(i, B=None, seed=None, b_offset=0):
     d["nsample"] = t["K"]
     d["spec"] = t
     return d
+
+
+def make_part_labels(B, N, num_parts, seed):
+    """Seeded labels of a multi-part segmentation batch, on CPU: shape_labels (B,) int64 in [0, S) and
+    points_labels (B,N) int64 with points_labels[b] < num_parts[shape_labels[b]]."""
+    g = torch.Generator().manual_seed(seed)
+    shape_labels = torch.randint(0, len(num_parts), (B,), generator=g)
+    u = torch.rand(B, N, generator=g)
+    limit = torch.tensor([num_parts[int(s)] for s in shape_labels], dtype=torch.float64)[:, None]
+    points_labels = (u.double() * limit).long().clamp_max(limit.long() - 1)
+    return dict(shape_labels=shape_labels, points_labels=points_labels)

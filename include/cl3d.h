@@ -279,6 +279,48 @@ int cl3d_pwmlp_bwd(const float* grad_out, const float* out, const float* ab_pm, 
                    int M, int K, int Cout, float radius, int training, float* scratch, float* dgamma_dbeta,
                    float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream, cl3d_stream_t side_stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Fused multi-shape part-segmentation head (multihead.cu).  Replaces the S per-shape heads of
+ * MultiPartSegHeadResNet (models/heads/segmentation_head.py:80-149), each
+ *     Conv1d(C,C,no bias) -> BatchNorm1d(C) -> ReLU -> Conv1d(C, num_parts[s]) + bias,
+ * all run over every point of x (B,C,N) channel-major.  Nothing of size S*C*B*N is materialised: BatchNorm
+ * statistics of every head follow from the channel means and one centred C x C second-moment matrix of x.
+ * Semantics of nn.BatchNorm1d in both modes (training: biased variance normalises, running statistics take the
+ * unbiased one, num_batches_tracked += 1, momentum < 0 means momentum=None; eval: running statistics).
+ *   desc_host    : host struct below (copied into kernel arguments: no device upload, CUDA-graph capturable)
+ *   w1 (S,C,C), gamma (S,C), beta (S,C), w2 (sum num_parts, C), b2 (sum num_parts): the heads' parameters
+ *                 concatenated over s
+ *   logits       : concatenation over s of contiguous (B, num_parts[s], N) blocks
+ *   save         : cl3d_mhead_save_floats(S,C) floats written by fwd, read by bwd
+ *   bwd          : desc_host->grad_logits[s] = d(loss)/d(logits of head s), (B,num_parts[s],N) contiguous, or NULL
+ *                  (counts as zero); grad_x (B,C,N) and every parameter gradient are fully written (no float atomics,
+ *                  fixed-order reductions: repeat runs are bit-identical).
+ * Limits: padded C <= 128, num_parts[s] <= 64, S <= 32; otherwise CL3D_ERR_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------------- */
+#define CL3D_MHEAD_MAX_HEADS 32
+#define CL3D_MHEAD_MAX_PARTS 64
+#define CL3D_MHEAD_MAX_CHANNELS 128
+typedef struct cl3d_mhead_desc {
+  int S;                                              /* number of heads (shape categories) */
+  int C;                                              /* channels of x */
+  int num_parts[CL3D_MHEAD_MAX_HEADS];                /* output channels of head s */
+  float* running_mean[CL3D_MHEAD_MAX_HEADS];          /* (C) per head: read in eval, updated in training */
+  float* running_var[CL3D_MHEAD_MAX_HEADS];
+  long long* num_batches_tracked[CL3D_MHEAD_MAX_HEADS]; /* per head, += 1 in training; may be NULL if momentum >= 0 */
+  const float* grad_logits[CL3D_MHEAD_MAX_HEADS];     /* backward only, see above */
+} cl3d_mhead_desc;
+size_t cl3d_mhead_save_floats(int S, int C);
+size_t cl3d_mhead_fwd_workspace_bytes(const cl3d_mhead_desc* desc_host, int B, int N);
+size_t cl3d_mhead_bwd_workspace_bytes(const cl3d_mhead_desc* desc_host, int B, int N);
+int cl3d_mhead_fwd(const cl3d_mhead_desc* desc_host, const float* x, int B, int N, const float* w1,
+                   const float* gamma, const float* beta, const float* w2, const float* b2, float eps,
+                   float momentum, int training, float* logits, float* save, void* workspace,
+                   size_t workspace_bytes, cl3d_stream_t stream);
+int cl3d_mhead_bwd(const cl3d_mhead_desc* desc_host, const float* x, int B, int N, const float* w1,
+                   const float* w2, const float* save, int training, float* grad_x, float* grad_w1,
+                   float* grad_gamma, float* grad_beta, float* grad_w2, float* grad_b2, void* workspace,
+                   size_t workspace_bytes, cl3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

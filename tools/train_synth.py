@@ -4,9 +4,11 @@
     python tools/train_synth.py --task classification --la pseudo_grid --batch 16 --points 10000
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29533 \
         tools/train_synth.py --task scene_segmentation --la pospool_sincos --batch 8 --points 15000
+    python tools/train_synth.py --task multi_part_segmentation --dataset shapenetpart --la pseudo_grid
 
 The reference's training step (function/train_modelnet_dist.py:254-297, train_s3dis_dist.py): forward, loss,
-zero_grad, backward, SGD step, under DistributedDataParallel(broadcast_buffers=False) (:206) -- with this package's
+zero_grad, backward, SGD step, under DistributedDataParallel(broadcast_buffers=False) (:206); part segmentation as function/train_partnet_dist.py:274-282 (multi-shape
+cross entropy on the list of per-shape logits, seeded shape and part labels) -- with this package's
 networks (closerlook3d_b200/backbone.py: the reference's module tree on the fused neighbourhood operators).
 Synthetic data (no datasets in the container): points on noisy unit-sphere shells (surface-like density, so the
 shipped cfgs' radii see realistic neighbour counts), xyz (+1) as input features as the datasets provide them.
@@ -43,10 +45,13 @@ def synth_batch(B, N, cin, seed, device, scale):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--task", default="classification", choices=["classification", "scene_segmentation"])
+    ap.add_argument("--task", default="classification", choices=["classification", "scene_segmentation",
+                                                                     "multi_part_segmentation"])
+    ap.add_argument("--dataset", default="partnet", choices=["partnet", "shapenetpart"],
+                    help="multi_part_segmentation: the PartNet or ShapeNetPart settings")
     ap.add_argument("--la", default="pseudo_grid", choices=sorted(LA))
-    ap.add_argument("--batch", type=int, default=None, help="clouds per GPU (default: the cfg's batch_size: 16 / 8)")
-    ap.add_argument("--points", type=int, default=None, help="points per cloud (default 10000 / 15000)")
+    ap.add_argument("--batch", type=int, default=None, help="clouds per GPU (default: the cfg's batch_size)")
+    ap.add_argument("--points", type=int, default=None, help="points per cloud (default: the cfg's num_points)")
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--ddp", action="store_true",
@@ -63,11 +68,13 @@ def main():
         dist.init_process_group("nccl", device_id=device)
     from closerlook3d_b200 import backbone as bb, pt_utils
     la, over = LA[args.la]
-    cfg = bb.model_config(args.task, la, **over)
-    B = args.batch or (16 if args.task == "classification" else 8)
+    part = args.task == "multi_part_segmentation"
+    cfg = bb.model_config(args.task, la, **over, **(dict(dataset=args.dataset) if part else {}))
+    B = args.batch or (cfg.batch_size if part else (16 if args.task == "classification" else 8))
     N = args.points or cfg.num_points
-    scale = 1.0 if args.task == "classification" else 2.0      # S3DIS spheres: in_radius 2 m
-    build = bb.build_classification if args.task == "classification" else bb.build_scene_segmentation
+    scale = 2.0 if args.task == "scene_segmentation" else 1.0      # S3DIS spheres: in_radius 2 m
+    build = {"classification": bb.build_classification, "scene_segmentation": bb.build_scene_segmentation,
+             "multi_part_segmentation": bb.build_multi_part_segmentation}[args.task]
     torch.manual_seed(0)
     model, criterion = build(cfg)
     model.init_weights()
@@ -84,14 +91,22 @@ def main():
     batches = [synth_batch(B, N, cfg.input_features_dim, 100 * rank + i, device, scale) for i in range(3)]
     if args.task == "classification":
         targets = [torch.randint(0, cfg.num_classes, (B,), device=device) for _ in batches]
+    elif part:
+        from closerlook3d_b200 import synth
+        labs = [synth.make_part_labels(B, N, cfg.num_parts, 100 * rank + i) for i in range(len(batches))]
+        targets = [(lab["points_labels"].to(device), lab["shape_labels"].to(device)) for lab in labs]
     else:
         targets = [torch.randint(0, cfg.num_classes, (B, N), device=device) for _ in batches]
 
     def step(i):
         xyz, mask, feats = batches[i % len(batches)]
         pred = net(xyz, mask, feats)
-        loss = criterion(pred, targets[i % len(batches)]) if args.task == "classification" else \
-            criterion(pred, targets[i % len(batches)], mask.float())
+        if args.task == "classification":
+            loss = criterion(pred, targets[i % len(batches)])
+        elif part:
+            loss = criterion(pred, *targets[i % len(batches)])
+        else:
+            loss = criterion(pred, targets[i % len(batches)], mask.float())
         if flat is not None:
             flat.zero()                 # the gradients are views of one buffer: one memset, one all-reduce
             loss.backward()
@@ -133,7 +148,7 @@ def main():
         fresh.load_state_dict(ck["model"], strict=True)
         ok = all(torch.equal(a.cpu(), b) for a, b in zip(model.state_dict().values(), fresh.state_dict().values()))
         print(json.dumps({"what": "whole-model training step (fwd + loss + bwd + SGD), synthetic clouds",
-                          "task": args.task, "local_aggregation": args.la, "n_gpus": world, "clouds_per_gpu": B,
+                          "task": args.task, **({"dataset": args.dataset} if part else {}), "local_aggregation": args.la, "n_gpus": world, "clouds_per_gpu": B,
                           "points_per_cloud": N, "steps": args.steps, "ms_per_step": ms_mean,
                           "ms_per_step_median": ms_median, "ms_slowest_step": ms_worst,
                           "points_per_s": B * N * world / (ms_mean * 1e-3),
