@@ -992,6 +992,7 @@ extern "C" int cl3d_agg_fwd(int family, int reduction, const float* feat_pm, con
   a.ntiles = B * ceil_div(M, kTile);
   a.arg_pm = arg_pm;
   if (reduction == CL3D_REDUCE_MAX) return aggmax_launch(family, a, false, a.ntiles, (cudaStream_t)stream_);
+  if (family == CL3D_FAM_PSEUDOGRID && pg3_fwd_supported(a)) return pg3_launch_fwd(a, (cudaStream_t)stream_);
   if (family == CL3D_FAM_PSEUDOGRID && pg2_supported(a)) return pg2_launch_fwd(a, (cudaStream_t)stream_);
   return dispatch_fwd(family, pick_ci(family, a.Cp), a, (cudaStream_t)stream_);
 }

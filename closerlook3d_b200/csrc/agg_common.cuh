@@ -94,10 +94,12 @@ __device__ __forceinline__ float family_weight(const LaneParams<FAM, CI>& lp, in
 int pg2_launch_fwd(const AggArgs& a, cudaStream_t stream);
 int pg2_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream);
 bool pg2_supported(const AggArgs& a);
-// third generation of the backward (tensor-core accumulation per kernel point) for the shapes pg3_supported accepts;
-// grid_x = rows of a.partial the caller sums
+// third generation (tensor-core accumulation per kernel point): forward for the shapes pg3_fwd_supported accepts,
+// backward for those of pg3_supported; backward: grid_x = rows of a.partial the caller sums
+int pg3_launch_fwd(const AggArgs& a, cudaStream_t stream);
 int pg3_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream);
 bool pg3_supported(const AggArgs& a);
+bool pg3_fwd_supported(const AggArgs& a);
 
 // agg_max.cu: max reduction for PosPool (xyz | sin_cos) and AdaptiveWeight
 int aggmax_launch(int family, const AggArgs& a, bool bwd, int grid_x, cudaStream_t stream);

@@ -1,5 +1,5 @@
 // pg.cu -- PseudoGrid (KPConv-like) local aggregation (sm_90a): second generation (forward and backward, any width)
-// and third generation (backward up to 128 channels: per-kernel-point sums on the tensor cores, see pg3_bwd_kernel).
+// and third generation (up to 128 channels: per-kernel-point sums on the tensor cores, see pg3_body).
 //
 // Reference: /root/reference/pytorch/models/local_aggregation_operators.py:384-419
 //     h[k',m]  = clamp(1 - |dp_m - K_k'| / extent, min 0)                (linear; 'constant': 1)
@@ -387,42 +387,47 @@ __global__ void __launch_bounds__(kPgWarps * 32, BWD ? 3 : 4) pg2_kernel(const A
 }
 
 // =================================================================================================
-// Third generation, backward: per centre point j the sums are regrouped per kernel point,
-//     U[k',c]     = sum_e h(k', s_j - q_e) * g[q_e,c]        a (16 x S) x (S x C) product, S = surviving entries
-//     d/df[j,c]   = sum_k' Wk[k',c] * U[k',c]
-//     d/dWk[k',c] += f[j,c] * U[k',c]                        in registers, over the warp's centre points
+// Third generation, both directions: per centre point the sums are regrouped per kernel point,
+//     U[k',c]     = sum_e h(k', e) * row_e[c]                a (16 x S) x (S x C) product, S = surviving entries
+//     out[p,c]    = sum_k' Wk[k',c] * U[k',c]                forward: agg (rows = features);  backward: d/df (rows = g)
+//     d/dWk[k',c] += f[j,c] * U[k',c]                        backward only, in registers over the warp's centre points
 // so the weight row and the d/dWk accumulator are touched once per (centre point, kernel point) in registers instead
 // of once per entry in shared memory.  U is computed on the tensor cores (mma.sync m16n8k8, 3xTF32 as gemm_tc.cuh:
 // every operand split into hi + lo TF32 halves, small terms first -- fp32 accuracy).  One warp per centre point:
 //   * staging as pg2 (lane = list entry, pg_influences), ballot-compacted; a surviving entry writes its dense
 //     h[16] row and its row offset into the warp's slot table, padded with zero rows to a multiple of 8 slots;
-//   * the surviving rows of g_pm go global -> shared with cp.async, 16 bytes per lane, all rows of the batch in
-//     flight at once (pad slots alias the first row: 0 * finite);
+//   * the surviving rows go global -> shared with cp.async, 16 bytes per lane, all rows of the batch in flight at once
+//     (pad slots alias the first row: 0 * finite);
 //   * per 8 slots and 8 channels: 2 B-fragment loads, 3 MMAs into the 4 accumulators of the tile;
-//   * epilogue in accumulator-fragment order; d/df summed over the 8 row groups of the warp by xor-shuffles.
-// A CTA serves a chunk of 8 * NT <= 72 channels (gridDim.y chunks of equal width).
+//   * epilogue in accumulator-fragment order; the sum over the 8 row groups of the warp by recursive halving;
+//   * the next centre point's chain -- list range, the lane's list entry, its coordinates -- is loaded into registers
+//     while the current one's rows are in flight, so a centre point starts with its influences.
+// A CTA serves a chunk of 8 * NT <= 72 channels (gridDim.y chunks of equal width) and loops over 32-centre tiles.
 // =================================================================================================
 constexpr int kPg3MaxNT = 9;     // 8-channel MMA tiles per chunk
 constexpr int kPg3Row = 72;      // words per staged row / weight row: == 8 (mod 32), B-fragment and Wk reads conflict-free
-constexpr int kPg3HRow = 24;     // words per slot-table row {h[16], row offset, -}: A-fragment reads conflict-free
+constexpr int kPg3HRow = 24;     // words per slot-table row {h[16], row offset, spare}: A-fragment reads conflict-free
+// The spare words of the slot table carry the next centre point's coordinates (pg3_fetch): words 17..19 of row 0 its
+// own, words 20..22 (even row r) or 21..23 (odd r) of row `lane` those of the lane's first list entry
+constexpr int kPg3CentreW = 17, kPg3NbrW = 20;
 constexpr int kPg3CtasPerSM = 2;
 
 struct Pg3Smem {
   size_t kp_off, wk_off, h_off, rows_off, own_off, out_off, total;
 };
-__host__ __device__ inline Pg3Smem pg3_smem() {
+__host__ __device__ inline Pg3Smem pg3_smem(bool bwd) {
   Pg3Smem L;
   size_t o = 0;
   L.kp_off = o;
   o += 3 * 8 * sizeof(u64);
   L.wk_off = o;
   o += (size_t)kMaxKP * kPg3Row * sizeof(float);
-  L.h_off = o;    // per warp [32][kPg3HRow]
+  L.h_off = o;    // per warp [32][kPg3HRow] (slot table, see kPg3CentreW)
   o += (size_t)kPgWarps * 32 * kPg3HRow * sizeof(float);
-  L.rows_off = o;  // per warp [32][kPg3Row]; at the end of the CTA: the warp's d/dWk sums [16][kPg3Row]
+  L.rows_off = o;  // per warp [32][kPg3Row]; at the end of a backward CTA: the warp's d/dWk sums [16][kPg3Row]
   o += (size_t)kPgWarps * 32 * kPg3Row * sizeof(float);
-  L.own_off = o;  // per warp [kPg3Row]: the centre point's own feature row
-  o += (size_t)kPgWarps * kPg3Row * sizeof(float);
+  L.own_off = o;  // backward, per warp [kPg3Row]: the centre point's own feature row
+  o += bwd ? (size_t)kPgWarps * kPg3Row * sizeof(float) : 0;
   L.out_off = o;
   o += (size_t)kPg3Row * (kPgTile + 1) * sizeof(float);
   L.total = align_up(o, 16);
@@ -433,6 +438,15 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
   uint32_t v;
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
   return v;
+}
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void cp_async4(uint32_t dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async8(uint32_t dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(dst), "l"(src) : "memory");
 }
 // D (16 x 8, fp32) += A (16 x 8, row) * B (8 x 8, col), TF32 operands
 __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -446,15 +460,166 @@ __device__ __forceinline__ void tf32_split(uint32_t x, uint32_t& hi, uint32_t& l
   lo = __float_as_uint(__uint_as_float(x) - __uint_as_float(hi));
 }
 
+// What a lane needs in registers to start a centre point: its list range and the row of its first list entry
+// (e0 + lane < e1).  The coordinates travel through the slot table's spare words (kPg3CentreW, kPg3NbrW).
+struct Pg3Next {
+  int e0, e1, r;
+};
+
+// Issues the loads of centre point pl of `tile` (an empty list past the last tile or the end of the cloud): list range
+// and entry into registers, the centre's and the entry's coordinates by cp.async into the slot table at h_a.  Always
+// commits exactly one cp.async group, empty or not, so that the caller's wait_group 1 leaves only this one pending.
+// Forward: centre = query, list = idx[q][0 .. ncount[q]); backward: centre = support point j, list = its transposed
+// entries q * K + k.
+template <bool BWD>
+__device__ __forceinline__ Pg3Next pg3_fetch(const AggArgs& a, int tile, int pl, int tiles_per_cloud, uint32_t h_a,
+                                             int lane) {
+  Pg3Next n = {0, 0, 0};
+  const int P = BWD ? a.N : a.M, R = BWD ? a.M : a.N;
+  const int b = tile / tiles_per_cloud, p = (tile % tiles_per_cloud) * kPgTile + pl;
+  if (tile >= a.ntiles || p >= P) {
+    cp_async_commit();
+    return n;
+  }
+  if (lane < 3)
+    cp_async4(h_a + (kPg3CentreW + lane) * 4, (BWD ? a.support_xyz : a.query_xyz) + ((size_t)b * P + p) * 3 + lane);
+  if constexpr (BWD) {
+    const int* off = a.csr_off + (size_t)b * (a.N + 1);
+    n.e0 = off[p];
+    n.e1 = off[p + 1];
+    if (n.e0 + lane < n.e1) n.r = a.csr_ent[(size_t)b * a.M * a.K + n.e0 + lane] / a.K;
+  } else {
+    const size_t gp = (size_t)b * a.M + p;
+    n.e1 = a.ncount[gp];
+    if (lane < n.e1) n.r = a.idx[gp * a.K + lane];
+  }
+  if (n.e0 + lane < n.e1) {  // 12 bytes in two requests, the 8-byte piece 8-byte aligned at both ends (as load_xyz)
+    const float* q = (BWD ? a.query_xyz : a.support_xyz) + ((size_t)b * R + n.r) * 3;
+    const uint32_t d = h_a + (uint32_t)(lane * kPg3HRow + kPg3NbrW + (n.r & 1)) * 4;
+    if (n.r & 1) {
+      cp_async4(d, q);
+      cp_async8(d + 4, q + 1);
+    } else {
+      cp_async8(d, q);
+      cp_async4(d + 8, q + 2);
+    }
+  }
+  cp_async_commit();
+  return n;
+}
+
+// Stages one batch of up to 32 list entries (lane = entry, relative position (dx, dy, dz), row offset roff) for the
+// tensor cores: evaluates the influences, ballot-compacts the entries with a non-zero influence into the warp's slot
+// table at h_a -- a dense h[16] row and the row offset per slot, padded with zero rows to a multiple of 8 slots --
+// and issues the cp.async of their rows into rows_a (2 * NT 16-byte pieces per row, 32 pieces per instruction) as
+// one committed group.  Returns the number of slots; 0 when no entry survived (nothing issued).
 template <int NT>
-__global__ void __launch_bounds__(kPgWarps * 32, kPg3CtasPerSM) pg3_bwd_kernel(const AggArgs a, int partial_rows) {
+__device__ __forceinline__ int pg3_stage(uint32_t h_a, uint32_t rows_a, const float* __restrict__ rows, bool valid, float dx,
+                                         float dy, float dz, unsigned roff, const u64* __restrict__ s_kx,
+                                         const u64* __restrict__ s_ky, const u64* __restrict__ s_kz, const AggArgs& a,
+                                         int lane) {
+  float h[kMaxKP];
+  pg_influences(h, valid, dx, dy, dz, s_kx, s_ky, s_kz, a.nkp, a.influence, a.inv_extent);
+  bool nz = false;
+#pragma unroll
+  for (int kp = 0; kp < kMaxKP; ++kp) nz |= h[kp] > 0.f;
+  const unsigned m = __ballot_sync(0xffffffffu, nz);
+  if (m == 0) return 0;
+  const int n = __popc(m), n8 = (n + 7) & ~7;
+  if (nz) {
+    const uint32_t d = h_a + (uint32_t)__popc(m & ((1u << lane) - 1u)) * (kPg3HRow * 4);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) sts_f4(d + 16 * q, make_float4(h[4 * q], h[4 * q + 1], h[4 * q + 2], h[4 * q + 3]));
+    sts_u32(d + 64, roff);
+  }
+  const unsigned roff0 = __shfl_sync(0xffffffffu, roff, __ffs(m) - 1);
+  if (lane >= n && lane < n8) {  // pad slots: zero influences, a valid row
+    const uint32_t d = h_a + (uint32_t)lane * (kPg3HRow * 4);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) sts_f4(d + 16 * q, make_float4(0.f, 0.f, 0.f, 0.f));
+    sts_u32(d + 64, roff0);
+  }
+  __syncwarp();
+  for (int id = lane; id < n8 * 2 * NT; id += 32) {
+    const int slot = id / (2 * NT), part = id % (2 * NT);
+    const unsigned ro = lds_u32(h_a + (uint32_t)slot * (kPg3HRow * 4) + 64);
+    cp_async16(rows_a + (uint32_t)(slot * kPg3Row + part * 4) * 4, row_at(rows, ro + 4u * part));
+  }
+  cp_async_commit();
+  return n8;
+}
+
+// U += h^T * rows over n8 staged slots (lane (g, t): A fragments from afrag_a, B fragments from bfrag_a)
+template <int NT>
+__device__ __forceinline__ void pg3_accumulate(float (&U)[NT][4], uint32_t afrag_a, uint32_t bfrag_a, int n8) {
+  for (int s = 0; s < n8; s += 8) {
+    uint32_t ah[4], al[4];
+    const uint32_t aa = afrag_a + (uint32_t)s * (kPg3HRow * 4);
+    tf32_split(lds_u32(aa), ah[0], al[0]);
+    tf32_split(lds_u32(aa + 8 * 4), ah[1], al[1]);
+    tf32_split(lds_u32(aa + 4 * kPg3HRow * 4), ah[2], al[2]);
+    tf32_split(lds_u32(aa + 4 * kPg3HRow * 4 + 8 * 4), ah[3], al[3]);
+    const uint32_t ba = bfrag_a + (uint32_t)s * (kPg3Row * 4);
+#pragma unroll
+    for (int i = 0; i < NT; ++i) {
+      uint32_t bh0, bl0, bh1, bl1;
+      tf32_split(lds_u32(ba + 32 * i), bh0, bl0);
+      tf32_split(lds_u32(ba + 32 * i + 4 * kPg3Row * 4), bh1, bl1);
+      mma_tf32(U[i], al, bh0, bh1);
+      mma_tf32(U[i], ah, bl0, bl1);
+      mma_tf32(U[i], ah, bh0, bh1);
+    }
+  }
+}
+
+// Sums v[0 .. V) over the 8 row groups of the warp (lane bits 2, 3, 4) by recursive halving: per level, a lane keeps
+// one half of its values and receives the partner's copy of that half, ceil(n / 2) shuffles for n values (17 for
+// V = 18, where an xor all-reduce takes 3 V = 54).  Partners pair by lane xor 4, then 8, then 16 -- the order of an
+// xor all-reduce with those offsets, so every sum is bit-identical to it.  On return s[j] is the sum of value
+// pg3_sum_index<V>(lane, j) when that is >= 0.
+template <int V>
+__device__ __forceinline__ void pg3_sum_rowgroups(const float (&v)[V], float (&s)[(V + 7) / 8], int lane) {
+  constexpr int H1 = (V + 1) / 2, H2 = (V + 3) / 4, H3 = (V + 7) / 8;
+  const bool b2 = lane & 4, b3 = lane & 8, b4 = lane & 16;
+  float w1[H1], w2[H2];
+#pragma unroll
+  for (int j = 0; j < H1; ++j) {
+    const float lo = v[j], hi = H1 + j < V ? v[H1 + j] : 0.f;
+    w1[j] = (b2 ? hi : lo) + __shfl_xor_sync(0xffffffffu, b2 ? lo : hi, 4);
+  }
+#pragma unroll
+  for (int j = 0; j < H2; ++j) {
+    const float lo = w1[j], hi = H2 + j < H1 ? w1[H2 + j] : 0.f;
+    w2[j] = (b3 ? hi : lo) + __shfl_xor_sync(0xffffffffu, b3 ? lo : hi, 8);
+  }
+#pragma unroll
+  for (int j = 0; j < H3; ++j) {
+    const float lo = w2[j], hi = H3 + j < H2 ? w2[H3 + j] : 0.f;
+    s[j] = (b4 ? hi : lo) + __shfl_xor_sync(0xffffffffu, b4 ? lo : hi, 16);
+  }
+}
+template <int V>
+__device__ __forceinline__ int pg3_sum_index(int lane, int j) {
+  constexpr int H1 = (V + 1) / 2, H2 = (V + 3) / 4, H3 = (V + 7) / 8;
+  const int r2 = (lane & 16 ? H3 : 0) + j;      // position among the level-2 values
+  const int r1 = (lane & 8 ? H2 : 0) + r2;      // among the level-1 values
+  const int r0 = (lane & 4 ? H1 : 0) + r1;      // among v
+  return r2 < H2 && r1 < H1 && r0 < V ? r0 : -1;  // else a padding slot
+}
+
+// BWD = false: centre = query q of cloud b, rows = feat_pm[idx[q][k]], k < ncount[q]; out[b,:,q] = agg and one
+//              BatchNorm partial row (sum, sum of squares over the tile's 32 queries) per tile.
+// BWD = true : centre = support point j, rows = g_pm[q_e] over the transposed list of j; out[b,:,j] = d/df and
+//              d/dWk in registers -> one partial row per CTA.
+template <bool BWD, int NT>
+__device__ __forceinline__ void pg3_body(const AggArgs& a, int partial_rows) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;  // MMA fragment coordinates
   constexpr int W = 8 * NT;               // channels of this CTA's chunk
   const int c0 = blockIdx.y * W;
   const int Cv = min(W, a.C - c0);  // real channels in it
-  const Pg3Smem L = pg3_smem();
+  const Pg3Smem L = pg3_smem(BWD);
   const u64* s_kx = reinterpret_cast<const u64*>(smem + L.kp_off);
   const u64* s_ky = s_kx + 8;
   const u64* s_kz = s_kx + 16;
@@ -472,194 +637,230 @@ __global__ void __launch_bounds__(kPgWarps * 32, kPg3CtasPerSM) pg3_bwd_kernel(c
   const uint32_t wk_a = smem_u32(smem + L.wk_off) + (uint32_t)(g * kPg3Row + 2 * t) * 4;
   const uint32_t afrag_a = h_a + (uint32_t)(t * kPg3HRow + g) * 4;
   const uint32_t bfrag_a = rows_a + (uint32_t)(t * kPg3Row + g) * 4;
-  const int tiles_per_cloud = (a.N + kPgTile - 1) / kPgTile;
+  const int P = BWD ? a.N : a.M;  // centre points per cloud
+  const int R = BWD ? a.M : a.N;  // rows of the gathered matrix per cloud
+  const int tiles_per_cloud = (P + kPgTile - 1) / kPgTile;
 
-  float dwk[NT][4];  // d/dWk of this warp's centre points, accumulator-fragment order
+  float dwk[BWD ? NT : 1][4];  // d/dWk of this warp's centre points, accumulator-fragment order
 #pragma unroll
-  for (int i = 0; i < NT; ++i) dwk[i][0] = dwk[i][1] = dwk[i][2] = dwk[i][3] = 0.f;
+  for (int i = 0; i < (BWD ? NT : 1); ++i) dwk[i][0] = dwk[i][1] = dwk[i][2] = dwk[i][3] = 0.f;
 
+  Pg3Next nxt = pg3_fetch<BWD>(a, blockIdx.x, warp, tiles_per_cloud, h_a, lane);
   for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
     const int b = tile / tiles_per_cloud;
     const int p0 = (tile % tiles_per_cloud) * kPgTile;
-    const float* rows = a.g_pm + (size_t)b * a.M * a.Cp + c0;
-    const float* cxyz = a.support_xyz + (size_t)b * a.N * 3;
-    const float* nxyz = a.query_xyz + (size_t)b * a.M * 3;
-    const int* off = a.csr_off + (size_t)b * (a.N + 1);
-    const int* list = a.csr_ent + (size_t)b * a.M * a.K;
+    const float* rows = (BWD ? a.g_pm : a.feat_pm) + (size_t)b * R * a.Cp + c0;
+    const float* nxyz = (BWD ? a.query_xyz : a.support_xyz) + (size_t)b * R * 3;
 
     for (int pl = warp; pl < kPgTile; pl += kPgWarps) {
       const int p = p0 + pl;
+      const Pg3Next cur = nxt;
+      // the warp's next centre point: the next one of this tile, else its first one of the CTA's next tile
+      const bool last = pl + kPgWarps >= kPgTile;
+      const int ntile = last ? tile + gridDim.x : tile, npl = last ? warp : pl + kPgWarps;
+      const int* list = BWD ? a.csr_ent + (size_t)b * a.M * a.K : a.idx + ((size_t)b * a.M + p) * a.K;
       float U[NT][4];
 #pragma unroll
       for (int i = 0; i < NT; ++i) U[i][0] = U[i][1] = U[i][2] = U[i][3] = 0.f;
       bool any = false;
-      if (p < a.N) {
-        const int e0 = off[p], e1 = off[p + 1];
-        const float cx = cxyz[p * 3 + 0], cy = cxyz[p * 3 + 1], cz = cxyz[p * 3 + 2];
-        if (e1 > e0 && lane < 2 * NT)  // own features (d/dWk), waited for with the first batch of rows
+      cp_async_wait<0>();  // this centre point's coordinates (pg3_fetch)
+      __syncwarp();
+      float cx = 0.f, cy = 0.f, cz = 0.f;
+      if (cur.e1 > cur.e0) {
+        cx = __uint_as_float(lds_u32(h_a + kPg3CentreW * 4));
+        cy = __uint_as_float(lds_u32(h_a + (kPg3CentreW + 1) * 4));
+        cz = __uint_as_float(lds_u32(h_a + (kPg3CentreW + 2) * 4));
+      }
+      if constexpr (BWD)
+        if (cur.e1 > cur.e0 && lane < 2 * NT)  // own features (d/dWk), waited for with the first batch of rows
           cp_async16(own_a + lane * 16, a.feat_pm + ((size_t)b * a.N + p) * a.Cp + c0 + lane * 4);
-        for (int eb = e0; eb < e1; eb += 32) {
-          const bool valid = eb + lane < e1;
-          float dx = 0.f, dy = 0.f, dz = 0.f;
-          unsigned roff = 0;
-          if (valid) {
-            const int r = list[eb + lane] / a.K;
-            float nx, ny, nz;
+      for (int eb = cur.e0; eb < cur.e1; eb += 32) {
+        const bool valid = eb + lane < cur.e1;
+        int r = cur.r;
+        float nx, ny, nz;
+        if (valid) {
+          if (eb == cur.e0) {
+            const uint32_t q = h_a + (uint32_t)(lane * kPg3HRow + kPg3NbrW + (r & 1)) * 4;
+            nx = __uint_as_float(lds_u32(q));
+            ny = __uint_as_float(lds_u32(q + 4));
+            nz = __uint_as_float(lds_u32(q + 8));
+          } else {  // later batches (lists longer than 32)
+            r = BWD ? list[eb + lane] / a.K : list[eb + lane];
             load_xyz(nxyz, r, nx, ny, nz);
-            dx = __fsub_rn(cx, nx), dy = __fsub_rn(cy, ny), dz = __fsub_rn(cz, nz);  // support - query
-            if (a.normalize) {
-              dx = __fmul_rn(dx, a.inv_radius);
-              dy = __fmul_rn(dy, a.inv_radius);
-              dz = __fmul_rn(dz, a.inv_radius);
-            }
-            roff = (unsigned)r * (unsigned)a.Cp;
           }
-          float h[kMaxKP];
-          pg_influences(h, valid, dx, dy, dz, s_kx, s_ky, s_kz, a.nkp, a.influence, a.inv_extent);
-          bool nz = false;
-#pragma unroll
-          for (int kp = 0; kp < kMaxKP; ++kp) nz |= h[kp] > 0.f;
-          const unsigned m = __ballot_sync(0xffffffffu, nz);
-          if (m == 0) continue;
-          const int n = __popc(m), n8 = (n + 7) & ~7;
-          if (nz) {
-            const uint32_t d = h_a + (uint32_t)__popc(m & ((1u << lane) - 1u)) * (kPg3HRow * 4);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) sts_f4(d + 16 * q, make_float4(h[4 * q], h[4 * q + 1], h[4 * q + 2], h[4 * q + 3]));
-            sts_f4(d + 64, make_float4(__uint_as_float(roff), 0.f, 0.f, 0.f));
-          }
-          const unsigned roff0 = __shfl_sync(0xffffffffu, roff, __ffs(m) - 1);
-          if (lane >= n && lane < n8) {  // pad slots: zero influences, a valid row
-            const uint32_t d = h_a + (uint32_t)lane * (kPg3HRow * 4);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) sts_f4(d + 16 * q, make_float4(0.f, 0.f, 0.f, 0.f));
-            sts_f4(d + 64, make_float4(__uint_as_float(roff0), 0.f, 0.f, 0.f));
-          }
-          __syncwarp();
-          // ---- rows of the surviving entries -> shared memory: 2 * NT 16-byte pieces per row, 32 pieces per instruction
-          for (int id = lane; id < n8 * 2 * NT; id += 32) {
-            const int slot = id / (2 * NT), part = id % (2 * NT);
-            const unsigned ro = lds_u32(h_a + (uint32_t)slot * (kPg3HRow * 4) + 64);
-            cp_async16(rows_a + (uint32_t)(slot * kPg3Row + part * 4) * 4, row_at(rows, ro + 4u * part));
-          }
-          cp_async_commit();
-          cp_async_wait<0>();
-          __syncwarp();
-          // ---- U += h^T * rows
-          for (int s = 0; s < n8; s += 8) {
-            uint32_t ah[4], al[4];
-            const uint32_t aa = afrag_a + (uint32_t)s * (kPg3HRow * 4);
-            tf32_split(lds_u32(aa), ah[0], al[0]);
-            tf32_split(lds_u32(aa + 8 * 4), ah[1], al[1]);
-            tf32_split(lds_u32(aa + 4 * kPg3HRow * 4), ah[2], al[2]);
-            tf32_split(lds_u32(aa + 4 * kPg3HRow * 4 + 8 * 4), ah[3], al[3]);
-            const uint32_t ba = bfrag_a + (uint32_t)s * (kPg3Row * 4);
-#pragma unroll
-            for (int i = 0; i < NT; ++i) {
-              uint32_t bh0, bl0, bh1, bl1;
-              tf32_split(lds_u32(ba + 32 * i), bh0, bl0);
-              tf32_split(lds_u32(ba + 32 * i + 4 * kPg3Row * 4), bh1, bl1);
-              mma_tf32(U[i], al, bh0, bh1);
-              mma_tf32(U[i], ah, bl0, bl1);
-              mma_tf32(U[i], ah, bh0, bh1);
-            }
-          }
-          any = true;
-          __syncwarp();  // the slot table and the rows are overwritten by the next batch
         }
+        float dx = 0.f, dy = 0.f, dz = 0.f;
+        unsigned roff = 0;
+        if (valid) {
+          // relative position = support - query in both directions (pt_utils.py:127)
+          if constexpr (BWD) {
+            dx = __fsub_rn(cx, nx), dy = __fsub_rn(cy, ny), dz = __fsub_rn(cz, nz);
+          } else {
+            dx = __fsub_rn(nx, cx), dy = __fsub_rn(ny, cy), dz = __fsub_rn(nz, cz);
+          }
+          if (a.normalize) {
+            dx = __fmul_rn(dx, a.inv_radius);
+            dy = __fmul_rn(dy, a.inv_radius);
+            dz = __fmul_rn(dz, a.inv_radius);
+          }
+          roff = (unsigned)r * (unsigned)a.Cp;
+        }
+        const int n8 = pg3_stage<NT>(h_a, rows_a, rows, valid, dx, dy, dz, roff, s_kx, s_ky, s_kz, a, lane);
+        const bool last = eb + 32 >= cur.e1;
+        if (last) nxt = pg3_fetch<BWD>(a, ntile, npl, tiles_per_cloud, h_a, lane);  // while the rows are in flight
+        if (n8 == 0) continue;
+        if (last)
+          cp_async_wait<1>();  // the rows; the next centre point's coordinates may still be in flight
+        else
+          cp_async_wait<0>();
+        __syncwarp();
+        pg3_accumulate<NT>(U, afrag_a, bfrag_a, n8);
+        any = true;
+        __syncwarp();  // the slot table and the rows are overwritten by the next batch
+      }
+      if (cur.e1 <= cur.e0) nxt = pg3_fetch<BWD>(a, ntile, npl, tiles_per_cloud, h_a, lane);
+      if constexpr (BWD) {
         cp_async_wait<0>();  // own row, when no batch had a surviving entry
         __syncwarp();
       }
       // ---- epilogue: lane (g, t) holds U[g][c], U[g][c+1], U[g+8][c], U[g+8][c+1] for c = 8i + 2t
+      float v[2 * NT];
 #pragma unroll
-      for (int i = 0; i < NT; ++i) {
-        float x = 0.f, y = 0.f;
-        if (any) {
+      for (int i = 0; i < 2 * NT; ++i) v[i] = 0.f;
+      if (any) {
+#pragma unroll
+        for (int i = 0; i < NT; ++i) {
           const float2 w0 = lds_f2(wk_a + 32 * i), w1 = lds_f2(wk_a + 32 * i + 8 * kPg3Row * 4);
-          const float2 f = lds_f2(own_a + (uint32_t)(8 * i + 2 * t) * 4);
-          x = fmaf(w1.x, U[i][2], w0.x * U[i][0]);
-          y = fmaf(w1.y, U[i][3], w0.y * U[i][1]);
-          dwk[i][0] = fmaf(f.x, U[i][0], dwk[i][0]);
-          dwk[i][1] = fmaf(f.y, U[i][1], dwk[i][1]);
-          dwk[i][2] = fmaf(f.x, U[i][2], dwk[i][2]);
-          dwk[i][3] = fmaf(f.y, U[i][3], dwk[i][3]);
-#pragma unroll
-          for (int o = 4; o < 32; o <<= 1) {
-            x += __shfl_xor_sync(0xffffffffu, x, o);
-            y += __shfl_xor_sync(0xffffffffu, y, o);
+          v[2 * i] = fmaf(w1.x, U[i][2], w0.x * U[i][0]);
+          v[2 * i + 1] = fmaf(w1.y, U[i][3], w0.y * U[i][1]);
+          if constexpr (BWD) {
+            const float2 f = lds_f2(own_a + (uint32_t)(8 * i + 2 * t) * 4);
+            dwk[i][0] = fmaf(f.x, U[i][0], dwk[i][0]);
+            dwk[i][1] = fmaf(f.y, U[i][1], dwk[i][1]);
+            dwk[i][2] = fmaf(f.x, U[i][2], dwk[i][2]);
+            dwk[i][3] = fmaf(f.y, U[i][3], dwk[i][3]);
           }
         }
-        if ((i & 7) == g) {  // every lane holds the sums: row group g writes tiles g and g + 8
-          s_out[(size_t)(8 * i + 2 * t) * (kPgTile + 1) + pl] = x;
-          s_out[(size_t)(8 * i + 2 * t + 1) * (kPgTile + 1) + pl] = y;
-        }
       }
-      __syncwarp();  // the own row is overwritten by the next centre point
+      float s[(2 * NT + 7) / 8];
+      pg3_sum_rowgroups<2 * NT>(v, s, lane);
+#pragma unroll
+      for (int j = 0; j < (2 * NT + 7) / 8; ++j) {
+        const int k = pg3_sum_index<2 * NT>(lane, j);  // value k = 2 i + (0: x, 1: y): channel 8 i + 2 t + (k & 1)
+        if (k >= 0) s_out[(size_t)(8 * (k >> 1) + 2 * t + (k & 1)) * (kPgTile + 1) + pl] = s[j];
+      }
+      if constexpr (BWD) __syncwarp();  // the own row is overwritten by the next centre point
     }
     __syncthreads();
-    // ---- tile -> channel-major (B,C,N)
+    // ---- tile -> channel-major (B,C,P)
     const int p = p0 + lane;
     for (int c = warp; c < Cv; c += kPgWarps)
-      if (p < a.N) a.out[((size_t)b * a.C + c0 + c) * a.N + p] = s_out[(size_t)c * (kPgTile + 1) + lane];
+      if (p < P) a.out[((size_t)b * a.C + c0 + c) * P + p] = s_out[(size_t)c * (kPgTile + 1) + lane];
+    if constexpr (!BWD) {
+      if (a.partial) {  // BatchNorm partial sums of the tile, over its 32 queries in order (absent ones hold 0)
+        for (int e = threadIdx.x; e < 2 * Cv; e += blockDim.x) {
+          const int s2 = e / Cv, c = e % Cv;
+          const float* o = s_out + (size_t)c * (kPgTile + 1);
+          float sum = 0.f;
+#pragma unroll
+          for (int q = 0; q < kPgTile; ++q) sum = s2 ? fmaf(o[q], o[q], sum) : sum + o[q];
+          a.partial[((size_t)tile * 2 + s2) * a.C + c0 + c] = sum;
+        }
+      }
+    }
     __syncthreads();
   }
-  // ---- d/dWk: the warps' sums in a fixed order -> one partial row per CTA: (gridDim.x, nkp, C); the rows of
-  // `partial` beyond gridDim.x (the caller sums cl3d_agg_bwd_num_blocks rows) are zero-filled
-  float* s_red = reinterpret_cast<float*>(smem + L.rows_off);
-  constexpr int kRedWarp = 32 * kPg3Row;  // floats between the warps' regions
+  if constexpr (BWD) {
+    // ---- d/dWk: the warps' sums in a fixed order -> one partial row per CTA: (gridDim.x, nkp, C); the rows of
+    // `partial` beyond gridDim.x (the caller sums cl3d_agg_bwd_num_blocks rows) are zero-filled
+    float* s_red = reinterpret_cast<float*>(smem + L.rows_off);
+    constexpr int kRedWarp = 32 * kPg3Row;  // floats between the warps' regions
 #pragma unroll
-  for (int i = 0; i < NT; ++i) {
-    float* d = s_red + (size_t)warp * kRedWarp + g * kPg3Row + 8 * i + 2 * t;
-    *reinterpret_cast<float2*>(d) = make_float2(dwk[i][0], dwk[i][1]);
-    *reinterpret_cast<float2*>(d + 8 * kPg3Row) = make_float2(dwk[i][2], dwk[i][3]);
-  }
-  __syncthreads();
-  for (int e = threadIdx.x; e < a.nkp * Cv; e += blockDim.x) {
-    const int kp = e / Cv, c = e % Cv;
-    float s = 0.f;
+    for (int i = 0; i < NT; ++i) {
+      float* d = s_red + (size_t)warp * kRedWarp + g * kPg3Row + 8 * i + 2 * t;
+      *reinterpret_cast<float2*>(d) = make_float2(dwk[i][0], dwk[i][1]);
+      *reinterpret_cast<float2*>(d + 8 * kPg3Row) = make_float2(dwk[i][2], dwk[i][3]);
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < a.nkp * Cv; e += blockDim.x) {
+      const int kp = e / Cv, c = e % Cv;
+      float s = 0.f;
 #pragma unroll
-    for (int w = 0; w < kPgWarps; ++w) s += s_red[(size_t)w * kRedWarp + kp * kPg3Row + c];
-    a.partial[((size_t)blockIdx.x * a.nkp + kp) * a.C + c0 + c] = s;
-    for (int row = gridDim.x + blockIdx.x; row < partial_rows; row += gridDim.x)
-      a.partial[((size_t)row * a.nkp + kp) * a.C + c0 + c] = 0.f;
+      for (int w = 0; w < kPgWarps; ++w) s += s_red[(size_t)w * kRedWarp + kp * kPg3Row + c];
+      a.partial[((size_t)blockIdx.x * a.nkp + kp) * a.C + c0 + c] = s;
+      for (int row = gridDim.x + blockIdx.x; row < partial_rows; row += gridDim.x)
+        a.partial[((size_t)row * a.nkp + kp) * a.C + c0 + c] = 0.f;
+    }
   }
+}
+
+template <int NT>
+__global__ void __launch_bounds__(kPgWarps * 32, kPg3CtasPerSM) pg3_fwd_kernel(const AggArgs a) {
+  pg3_body<false, NT>(a, 0);
+}
+template <int NT>
+__global__ void __launch_bounds__(kPgWarps * 32, kPg3CtasPerSM) pg3_bwd_kernel(const AggArgs a, int partial_rows) {
+  pg3_body<true, NT>(a, partial_rows);
 }
 
 // ---------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------
-// Third generation (backward): up to 72 padded channels in one chunk, or two equal chunks up to 128.
-// CL3D_PG_V2 forces the second generation (A/B measurements, tests).
+// Third generation: up to 72 padded channels in one chunk, or two equal chunks up to 128.
+// CL3D_PG_V2 forces the second generation in both directions (A/B measurements, tests).
 static int pg3_num_chunks(int Cp) { return Cp <= 8 * kPg3MaxNT ? 1 : 2; }
 bool pg3_supported(const AggArgs& a) {
   if (getenv("CL3D_PG_V1") || getenv("CL3D_PG_V2")) return false;
   if (a.nkp < 1 || a.nkp > kMaxKP || a.Cp > 128) return false;
   return a.Cp % (8 * pg3_num_chunks(a.Cp)) == 0;
 }
+// The forward takes the third generation only up to 40 padded channels: measured on H100 (DESIGN.md 7.1) it beats
+// pg2_kernel<false> at 36 channels but loses at 72 and 128, where its row staging at 2 CTAs per SM costs more than
+// pg2's weight-row loads at 4.
+constexpr int kPg3FwdMaxCp = 40;
+bool pg3_fwd_supported(const AggArgs& a) { return a.Cp <= kPg3FwdMaxCp && pg3_supported(a); }
 
-template <int NT>
+template <bool BWD, int NT>
 static void pg3_launch_nt(const AggArgs& a, dim3 grid, int partial_rows, cudaStream_t stream) {
   static std::atomic<unsigned long long> seen{0};
-  allow_big_smem(pg3_bwd_kernel<NT>, seen);
-  pg3_bwd_kernel<NT><<<grid, kPgWarps * 32, pg3_smem().total, stream>>>(a, partial_rows);
+  if constexpr (BWD) {
+    allow_big_smem(pg3_bwd_kernel<NT>, seen);
+    pg3_bwd_kernel<NT><<<grid, kPgWarps * 32, pg3_smem(true).total, stream>>>(a, partial_rows);
+  } else {
+    allow_big_smem(pg3_fwd_kernel<NT>, seen);
+    pg3_fwd_kernel<NT><<<grid, kPgWarps * 32, pg3_smem(false).total, stream>>>(a);
+  }
+}
+
+template <bool BWD>
+static void pg3_launch(const AggArgs& a, dim3 grid, int partial_rows, cudaStream_t stream) {
+  switch (a.Cp / (8 * pg3_num_chunks(a.Cp))) {
+    case 1: pg3_launch_nt<BWD, 1>(a, grid, partial_rows, stream); break;
+    case 2: pg3_launch_nt<BWD, 2>(a, grid, partial_rows, stream); break;
+    case 3: pg3_launch_nt<BWD, 3>(a, grid, partial_rows, stream); break;
+    case 4: pg3_launch_nt<BWD, 4>(a, grid, partial_rows, stream); break;
+    case 5: pg3_launch_nt<BWD, 5>(a, grid, partial_rows, stream); break;
+    case 6: pg3_launch_nt<BWD, 6>(a, grid, partial_rows, stream); break;
+    case 7: pg3_launch_nt<BWD, 7>(a, grid, partial_rows, stream); break;
+    case 8: pg3_launch_nt<BWD, 8>(a, grid, partial_rows, stream); break;
+    default: pg3_launch_nt<BWD, 9>(a, grid, partial_rows, stream); break;
+  }
+}
+
+// one wave of resident CTAs looping over the 32-query tiles (CL3D_TEST_MAX_GRID caps it)
+int pg3_launch_fwd(const AggArgs& a, cudaStream_t stream) {
+  if (!pg3_fwd_supported(a)) return CL3D_ERR_UNSUPPORTED;
+  const int gx = max(1, min(a.ntiles, min(kPg3CtasPerSM * sm_count(), persistent_grid_cap())));
+  pg3_launch<false>(a, dim3(gx, pg3_num_chunks(a.Cp)), 0, stream);
+  CL3D_LAUNCHED(1);
+  return check_launch("pg3_fwd_kernel");
 }
 
 // grid_x = rows of a.partial the caller sums; the kernel runs one wave of resident CTAs
 int pg3_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
   if (!pg3_supported(a)) return CL3D_ERR_UNSUPPORTED;
-  const int nchunks = pg3_num_chunks(a.Cp);
-  const dim3 grid(min(grid_x, kPg3CtasPerSM * sm_count()), nchunks);
-  switch (a.Cp / (8 * nchunks)) {
-    case 1: pg3_launch_nt<1>(a, grid, grid_x, stream); break;
-    case 2: pg3_launch_nt<2>(a, grid, grid_x, stream); break;
-    case 3: pg3_launch_nt<3>(a, grid, grid_x, stream); break;
-    case 4: pg3_launch_nt<4>(a, grid, grid_x, stream); break;
-    case 5: pg3_launch_nt<5>(a, grid, grid_x, stream); break;
-    case 6: pg3_launch_nt<6>(a, grid, grid_x, stream); break;
-    case 7: pg3_launch_nt<7>(a, grid, grid_x, stream); break;
-    case 8: pg3_launch_nt<8>(a, grid, grid_x, stream); break;
-    default: pg3_launch_nt<9>(a, grid, grid_x, stream); break;
-  }
+  const dim3 grid(min(grid_x, kPg3CtasPerSM * sm_count()), pg3_num_chunks(a.Cp));
+  pg3_launch<true>(a, grid, grid_x, stream);
   CL3D_LAUNCHED(1);
   return check_launch("pg3_bwd_kernel");
 }

@@ -1,0 +1,111 @@
+"""Third-generation PseudoGrid forward (csrc/pg.cu pg3_fwd_kernel: per-kernel-point sums U = h^T f on the tensor cores
+with 3xTF32, then out = sum_k' Wk * U) against the second-generation kernel (CL3D_PG_V2=1) on the same inputs and
+lists, and both against a float64 evaluation of the same sums.  Same terms and the same influences; the sums are
+regrouped, so the comparison is to rounding, not bit for bit.  The BatchNorm partial rows keep their meaning: the sum
+and the sum of squares of the output over each tile of 32 queries.  The forward takes the third generation up to 40
+padded channels (C = 8, 36 below); the wider cases check that the dispatch still computes the same sums."""
+import pytest
+import torch
+
+from closerlook3d_b200 import ops
+from test_pg_v3_gpu import CASES, _case, _err, env
+
+pytestmark = pytest.mark.gpu
+
+
+def _fwd(c, influence):
+    xyz = c["g"]["xyz"]
+    agg, part = ops.agg_fwd(ops.FAM_PSEUDOGRID, ops.REDUCE["sum"], c["feat_pm"], xyz, xyz, c["idx"], c["ncount"],
+                            c["kpts"], c["wk"], c["C"], c["r"], 0, 1, c["nkp"], c["extent"], influence)
+    torch.cuda.synchronize()
+    return agg, part
+
+
+def _f64(c, influence):
+    """agg (B,C,M) in float64 from the fp32 relative positions (gather of oracle.f64_ext)"""
+    from oracle import f64_ext
+    xyz, idx, K = c["g"]["xyz"], c["idx"], c["K"]
+    sx = f64_ext.group_points(xyz.transpose(1, 2).contiguous(), idx)            # (B,3,M,K)
+    dp = (sx - xyz.transpose(1, 2)[..., None]).permute(0, 2, 3, 1)               # support - query, fp32
+    if influence == 1:
+        h = torch.ones(*dp.shape[:3], c["nkp"], dtype=torch.float64, device=dp.device)
+    else:
+        dist = (dp[..., None, :].double() - c["kpts"].double()).pow(2).sum(-1).sqrt()
+        h = (1.0 - dist / c["extent"]).clamp(min=0.0)                            # (B,M,K,nkp)
+    h = h * (torch.arange(K, device=dp.device)[None, None, :] < c["ncount"][..., None])[..., None]
+    fj = f64_ext.group_points(c["g"]["features"].double(), idx)                  # (B,C,M,K)
+    return torch.einsum("bmkp,pc,bcmk->bcm", h, c["wk"].double(), fj)
+
+
+def _tile_sums(agg):
+    """(ntiles, 2, C) float64: sum and sum of squares of agg over each tile of 32 queries of each cloud"""
+    B, C, M = agg.shape
+    T = (M + 31) // 32
+    x = torch.zeros(B, C, T * 32, dtype=torch.float64, device=agg.device)
+    x[..., :M] = agg.double()
+    x = x.view(B, C, T, 32)
+    return torch.stack([x.sum(-1), (x * x).sum(-1)], -1).permute(0, 2, 3, 1).reshape(B * T, 2, C)   # row b * T + t
+
+
+@pytest.mark.parametrize("B,N,K,C,nkp,influence,thin", CASES)
+@pytest.mark.parametrize("max_grid", [0, 5])
+def test_pg_v3_fwd_matches_v2_and_f64(cuda, B, N, K, C, nkp, influence, thin, max_grid):
+    c = _case(cuda, B, N, K, C, nkp, 91 + N + C, thin)
+    if K > 32:
+        assert int(c["ncount"].max()) > 32                                       # several batches per query
+    grid = dict(CL3D_TEST_MAX_GRID=max_grid) if max_grid else {}            # 5 CTAs: every CTA loops over many tiles
+    with env(**grid):
+        with env(CL3D_PG_V2=1):
+            a2, p2 = _fwd(c, influence)
+        a3, p3 = _fwd(c, influence)
+        a3b, p3b = _fwd(c, influence)
+    assert torch.equal(a3, a3b) and torch.equal(p3, p3b), "two runs of the same grid differ"
+    assert _err(a3, a2) <= 1e-5, f"agg: v3 differs from v2 by {_err(a3, a2):.2e}"
+    assert p3.shape == p2.shape
+    assert _err(p3, p2) <= 1e-5, f"BatchNorm partials: v3 differs from v2 by {_err(p3, p2):.2e}"
+    ref = _f64(c, influence)
+    e2, e3 = _err(a2, ref), _err(a3, ref)
+    ep = _err(p3, _tile_sums(ref))
+    print(f"float64 reference: agg v2 {e2:.2e} v3 {e3:.2e} | v3 BatchNorm partials {ep:.2e}")
+    assert e3 <= max(3 * e2, 2e-6), f"v3 {e3:.2e} against v2 {e2:.2e}"
+    assert ep <= 1e-5
+    # BatchNorm statistics from the partial rows, as cl3d_bn_finalize sums them
+    s2, s3 = p2.double().sum(0), p3.double().sum(0)
+    assert float((s3 - s2).abs().max()) <= 1e-5 * max(1.0, float(s2.abs().max()))
+
+
+def test_pg_v3_fwd_graph_replay_equals_eager(cuda):
+    c = _case(cuda, 2, 3000, 26, 72, 15, 17)
+    eager = _fwd(c, 0)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        _fwd(c, 0)
+    torch.cuda.current_stream().wait_stream(s)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        xyz = c["g"]["xyz"]
+        out = ops.agg_fwd(ops.FAM_PSEUDOGRID, ops.REDUCE["sum"], c["feat_pm"], xyz, xyz, c["idx"], c["ncount"],
+                          c["kpts"], c["wk"], c["C"], c["r"], 0, 1, c["nkp"], c["extent"], 0)
+    out[0].zero_()
+    out[1].zero_()
+    graph.replay()
+    torch.cuda.synchronize()
+    assert torch.equal(out[0], eager[0]) and torch.equal(out[1], eager[1])
+
+
+def test_pg_v3_fwd_dispatch(cuda):
+    """up to 40 padded channels the forward takes pg3_fwd_kernel: its sums are regrouped, so its bits differ from the
+    second generation's (CL3D_PG_V2=1); bench.py's default shape (S3DIS PseudoGrid: B=8, N=15000, K=26, C=72) keeps the
+    second-generation forward, where it measured faster, so its bits are those of CL3D_PG_V2=1"""
+    narrow = _case(cuda, 8, 15000, 26, 36, 15, 3)
+    with env(CL3D_PG_V2=1):
+        a2, _ = _fwd(narrow, 0)
+    a3, _ = _fwd(narrow, 0)
+    assert not torch.equal(a2, a3)
+    assert _err(a3, a2) <= 1e-5
+    c3 = _case(cuda, 8, 15000, 26, 72, 15, 3)
+    with env(CL3D_PG_V2=1):
+        a2, p2 = _fwd(c3, 0)
+    a3, p3 = _fwd(c3, 0)
+    assert torch.equal(a2, a3) and torch.equal(p2, p3)

@@ -1,13 +1,14 @@
-"""A/B of the PseudoGrid backward generations on one GPU: the third-generation kernel (default) against the second
-(CL3D_PG_V2=1), the arms alternated inside one process.
+"""A/B of the PseudoGrid kernel generations on one GPU, forward and backward: the third-generation kernels (default)
+against the second (CL3D_PG_V2=1), the arms alternated inside one process.
 
     python tools/bench_pg.py [--launches 200] [--rounds 5]
 
 Per shape: inputs from synth.make_cloud_batch, lists from ops.ball_query + ops.build_csr, a ring of batches larger
 than L2 so no launch finds its inputs there; ops.agg_bwd timed with CUDA events over `launches` calls per arm and
-round after a warm-up (the library's per-entry-point profiler: events around cl3d_agg_bwd alone).  Prints, per shape
-and arm, the median and the min..max over the rounds (ms per call), and the ratio of the medians.  The forward (one
-generation) is timed the same way for scale.  Needs a GPU; prints the card and its power limit.
+round after a warm-up (the library's per-entry-point profiler: events around cl3d_agg_fwd / cl3d_agg_bwd alone).
+Prints, per shape, direction and arm, the median and the min..max over the rounds (ms per call), and the ratio of the
+medians; for the c3 shape also the layout pass (cl3d_to_point_major of the features), which sits on the same step's
+critical path.  Needs a GPU; prints the card, its power limit and maximum SM clock.
 """
 import argparse
 import os
@@ -80,19 +81,24 @@ def main():
             return ops.agg_fwd(ops.FAM_PSEUDOGRID, ops.REDUCE["sum"], b["feat_pm"], b["xyz"], b["xyz"], b["idx"], b["ncount"],
                                kpts, wk, C, r, 0, 1, 15, 0.4 * r, 0)
 
-        t = {"v2": [], "v3": []}
-        for _ in range(args.rounds):
-            os.environ["CL3D_PG_V2"] = "1"
-            try:
-                t["v2"].append(timed(bwd, "cl3d_agg_bwd", ring, args.launches))
-            finally:
-                del os.environ["CL3D_PG_V2"]
-            t["v3"].append(timed(bwd, "cl3d_agg_bwd", ring, args.launches))
-        tf = [timed(fwd, "cl3d_agg_fwd", ring, args.launches) for _ in range(2)]
-        m2, m3 = statistics.median(t["v2"]), statistics.median(t["v3"])
-        print(f"{name}: bwd v2 {m2:.4f} ms [{min(t['v2']):.4f}..{max(t['v2']):.4f}]  "
-              f"v3 {m3:.4f} ms [{min(t['v3']):.4f}..{max(t['v3']):.4f}]  v2/v3 = {m2 / m3:.2f}x  "
-              f"| fwd {min(tf):.4f} ms", flush=True)
+        for what, fn, entry in (("fwd", fwd, "cl3d_agg_fwd"), ("bwd", bwd, "cl3d_agg_bwd")):
+            t = {"v2": [], "v3": []}
+            for _ in range(args.rounds):
+                os.environ["CL3D_PG_V2"] = "1"
+                try:
+                    t["v2"].append(timed(fn, entry, ring, args.launches))
+                finally:
+                    del os.environ["CL3D_PG_V2"]
+                t["v3"].append(timed(fn, entry, ring, args.launches))
+            m2, m3 = statistics.median(t["v2"]), statistics.median(t["v3"])
+            print(f"{name}: {what} v2 {m2:.4f} ms [{min(t['v2']):.4f}..{max(t['v2']):.4f}]  "
+                  f"v3 {m3:.4f} ms [{min(t['v3']):.4f}..{max(t['v3']):.4f}]  v2/v3 = {m2 / m3:.2f}x", flush=True)
+        if name.startswith("c3  B=8"):
+            feats = [torch.randn(B, C, N, device=dev) for _ in range(2)]
+            tl = [timed(lambda f: ops.to_point_major(f), "cl3d_to_point_major", feats, args.launches)
+                  for _ in range(args.rounds)]
+            print(f"{name}: cl3d_to_point_major {statistics.median(tl):.4f} ms [{min(tl):.4f}..{max(tl):.4f}]",
+                  flush=True)
 
 
 if __name__ == "__main__":
