@@ -431,58 +431,38 @@ __device__ __forceinline__ u64 make_key(float d2, int idx) {
   return ((u64)__float_as_uint(d2) << 32) | (unsigned)idx;  // d2 >= +0 -> bit pattern is monotone
 }
 
-// Warp bitonic sort of up to 32*E 64-bit keys (element i = e*32 + lane), ascending; missing elements = ~0.
+// s_sorted[rank of L[i]] = index of L[i] for every rank < K.  A lane ranks E keys (i = base + e*32 + lane) per pass
+// over the list, so each broadcast load serves E compares and the E counts are independent dependency chains.
 template <int E>
-__device__ __forceinline__ void warp_bitonic_sort(u64 (&key)[E]) {
+__device__ __forceinline__ void rank_keys(const u64* L, int cnt, int* s_sorted, int K) {
   const int lane = lane_id();
-  constexpr int n = 32 * E;
+  for (int base = 0; base < cnt; base += 32 * E) {
+    u64 my[E];
+    int rho[E];
 #pragma unroll
-  for (int k = 2; k <= n; k <<= 1) {
-#pragma unroll
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      if (j >= 32) {  // partner lives in another register of the same lane
-        const int de = j >> 5;
-#pragma unroll
-        for (int e = 0; e < E; ++e) {
-          if ((e & de) == 0) {
-            const bool up = (((e * 32 + lane) & k) == 0);
-            const u64 a = key[e], b = key[e | de];
-            const bool sw = (a > b) == up;
-            key[e] = sw ? b : a;
-            key[e | de] = sw ? a : b;
-          }
-        }
-      } else {
-#pragma unroll
-        for (int e = 0; e < E; ++e) {
-          const u64 other = __shfl_xor_sync(0xffffffffu, key[e], j);
-          const bool up = (((e * 32 + lane) & k) == 0);
-          const bool lower = ((lane & j) == 0);
-          const u64 mn = other < key[e] ? other : key[e], mx = other < key[e] ? key[e] : other;
-          key[e] = (lower == up) ? mn : mx;
-        }
-      }
+    for (int e = 0; e < E; ++e) {
+      const int i = base + e * 32 + lane;
+      my[e] = i < cnt ? L[i] : ~0ull;
+      rho[e] = 0;
     }
-  }
-}
-
-template <int E>
-__device__ __forceinline__ void emit_sorted(const u64* L, int cnt, int* s_sorted, int K) {
-  const int lane = lane_id();
-  u64 key[E];
+#pragma unroll 4
+    for (int j = 0; j < cnt; ++j) {
+      const u64 v = L[j];
 #pragma unroll
-  for (int e = 0; e < E; ++e) key[e] = (e * 32 + lane) < cnt ? L[e * 32 + lane] : ~0ull;
-  warp_bitonic_sort<E>(key);
+      for (int e = 0; e < E; ++e) rho[e] += (v < my[e]) ? 1 : 0;
+    }
 #pragma unroll
-  for (int e = 0; e < E; ++e) {
-    const int i = e * 32 + lane;
-    if (i < cnt && i < K) s_sorted[i] = (int)(unsigned)(key[e] & 0xffffffffu);
+    for (int e = 0; e < E; ++e)
+      if (base + e * 32 + lane < cnt && rho[e] < K) s_sorted[rho[e]] = (int)(unsigned)(my[e] & 0xffffffffu);
   }
 }
 
 // L[0..cnt) holds the reference's candidate list (any order; unique indices).  Emits the first K of the list
 // sorted by (d2, index) -- identical to the reference's stable sort of an index-ascending list
 // (masked_ordered_ball_query_gpu.cu:77) -- then the cyclic padding (:83-86) and masks (:79-93).
+// Selection by counting: the keys are unique, so a key's place in the sorted list is the number of smaller keys.  Each
+// lane ranks the keys it holds against the whole list (broadcast shared-memory loads, cnt * ceil(cnt/32) compares
+// per lane) and writes the ones that land below K -- one loop for every cnt <= 3K, no sorting network.
 // csr_cnt (may be null): per-support-point reference counters of this cloud.  Every counted slot (k < ncount, or all K
 // slots with csr_all) takes its rank inside the support point's transposed list right here (one int atomic per
 // slot, K of them in flight per warp), so the list build that follows is a scan and an atomic-free scatter.
@@ -491,20 +471,10 @@ __device__ __forceinline__ void emit_query(const u64* L, int cnt, int* s_sorted,
                                            int* __restrict__ csr_cnt = nullptr, int* __restrict__ rank_out = nullptr,
                                            int csr_all = 0) {
   const int lane = lane_id();
-  if (cnt <= 32) {
-    emit_sorted<1>(L, cnt, s_sorted, K);
-  } else if (cnt <= 64) {
-    emit_sorted<2>(L, cnt, s_sorted, K);
-  } else if (cnt <= 128) {
-    emit_sorted<4>(L, cnt, s_sorted, K);
-  } else {  // rank by counting (O(cnt^2/32)); only reached for nsample > 42
-    for (int i = lane; i < cnt; i += 32) {
-      const u64 my = L[i];
-      int rho = 0;
-      for (int j = 0; j < cnt; ++j) rho += (L[j] < my) ? 1 : 0;
-      if (rho < K) s_sorted[rho] = (int)(unsigned)(my & 0xffffffffu);
-    }
-  }
+  if (cnt <= 32)
+    rank_keys<1>(L, cnt, s_sorted, K);
+  else
+    rank_keys<2>(L, cnt, s_sorted, K);
   __syncwarp();
   const int ncnt = qm != 0 ? (cnt < K ? cnt : K) : K;
   for (int k = lane; k < K; k += 32) {
@@ -644,11 +614,12 @@ __global__ void __launch_bounds__(kBQWarps * 32) ball_query_brute_kernel(
 // ---------------------------------------------------------------------------------------------
 // grid kernel: one warp per query, 9 contiguous cell-row ranges
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kBQWarps * 32) ball_query_grid_kernel(
+__global__ void __launch_bounds__(kBQWarps * 32, 5) ball_query_grid_kernel(
     const float* __restrict__ query_xyz, const float* __restrict__ support_xyz, const int* __restrict__ query_mask,
     const GridParams* __restrict__ params, const int* __restrict__ cell_start, const float4* __restrict__ sorted,
-    int B, int N, int M, float radius, int K, int cell_cap, int* __restrict__ idx, int* __restrict__ idx_mask,
-    int* __restrict__ ncount, int* __restrict__ csr_cnt, int* __restrict__ csr_rank, int csr_all) {
+    int B, int N, int M, float radius, int K, int cell_cap, int cell_order, int* __restrict__ idx,
+    int* __restrict__ idx_mask, int* __restrict__ ncount, int* __restrict__ csr_cnt, int* __restrict__ csr_rank,
+    int csr_all) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int cap3k = 3 * K;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -656,16 +627,32 @@ __global__ void __launch_bounds__(kBQWarps * 32) ball_query_grid_kernel(
   u64* s_keep = reinterpret_cast<u64*>(smem_raw) + (size_t)kBQWarps * kCandCap + (size_t)warp * cap3k;
   int* s_sorted = reinterpret_cast<int*>(reinterpret_cast<u64*>(smem_raw) + (size_t)kBQWarps * (kCandCap + cap3k)) +
                   (size_t)warp * K;
-  const long long gq = (long long)blockIdx.x * kBQWarps + warp;
-  if (gq >= (long long)B * M) return;
-  const int b = (int)(gq / M);
+  const long long gw = (long long)blockIdx.x * kBQWarps + warp;
+  if (gw >= (long long)B * M) return;
+  const int b = (int)(gw / M);
   const GridParams p = params[b];
-  const float* qp = query_xyz + (size_t)gq * 3;
-  const float qx = qp[0], qy = qp[1], qz = qp[2];
+  const float4* pts = sorted + (size_t)b * N;
+  // Query set == support set (cell_order): warp w takes the w-th valid point in cell order, so the warps of a CTA and
+  // the CTAs resident beside it walk the same cells and find their candidates in L1.  The padded rows past the valid
+  // prefix still get lists; they follow in index order.
+  int q = (int)(gw - (long long)b * M);
+  float qx, qy, qz;
+  if (cell_order && q < p.n_valid) {
+    const float4 c = pts[q];
+    q = __float_as_int(c.w);
+    qx = c.x;
+    qy = c.y;
+    qz = c.z;
+  } else {
+    const float* qp = query_xyz + ((size_t)b * M + q) * 3;
+    qx = qp[0];
+    qy = qp[1];
+    qz = qp[2];
+  }
+  const size_t gq = (size_t)b * M + q;
   const float r2 = __fmul_rn(radius, radius);
   const unsigned lt = (1u << lane) - 1u;
   const int* cs = cell_start + (size_t)b * (cell_cap + 1);
-  const float4* pts = sorted + (size_t)b * N;
 
   // query cell (may lie outside the support's bounding box)
   float fx = floorf((qx - p.ox) * p.inv_h), fy = floorf((qy - p.oy) * p.inv_h), fz = floorf((qz - p.oz) * p.inv_h);
@@ -675,84 +662,96 @@ __global__ void __launch_bounds__(kBQWarps * 32) ball_query_grid_kernel(
   const int cx = (int)fx, cy = (int)fy, cz = (int)fz;
   const int x0 = max(cx - 1, 0), x1 = min(cx + 1, p.gx - 1);
 
-  int T = 0;
-  u64 best = ~0ull;
-  if (p.n_valid > 0 && x0 <= x1) {
-    for (int dz = -1; dz <= 1; ++dz) {
-      const int z = cz + dz;
-      if (z < 0 || z >= p.gz) continue;
-      for (int dy = -1; dy <= 1; ++dy) {
-        const int y = cy + dy;
-        if (y < 0 || y >= p.gy) continue;
-        const int row = p.gx * (y + p.gy * z);
-        const int s = cs[row + x0], e = cs[row + x1 + 1];
-        for (int base = s; base < e; base += 32) {
-          const int i = base + lane;
-          bool in = false;
-          u64 key = 0;
-          if (i < e) {
-            const float4 c = pts[i];
-            const float d2 = ref_d2(qx, qy, qz, c.x, c.y, c.z);
-            in = d2 < r2;
-            key = make_key(d2, __float_as_int(c.w));
-          }
-          const unsigned m = __ballot_sync(0xffffffffu, in);
-          if (in) {
-            const int pos = T + __popc(m & lt);
-            if (pos < kCandCap) s_cand[pos] = key;
-            best = key < best ? key : best;
-          }
-          T += __popc(m);
-        }
-      }
+  // The 9 (dz, dy) rows of the 27 cells: lane r < 9 loads row r's [start, end) -- all 18 loads in flight together --
+  // and a 9-lane scan lays the rows end to end, so the candidates are one range [0, total) walked in full 32-lane
+  // chunks.  Position i belongs to the last row whose offset is <= i (empty rows share their successor's offset).
+  int st = 0, len = 0;
+  if (lane < 9 && p.n_valid > 0 && x0 <= x1) {
+    const int z = cz + lane / 3 - 1, y = cy + lane % 3 - 1;
+    if (z >= 0 && z < p.gz && y >= 0 && y < p.gy) {
+      const int row = p.gx * (y + p.gy * z);
+      st = cs[row + x0];
+      len = cs[row + x1 + 1] - st;
     }
   }
+  int incl = len;
+#pragma unroll
+  for (int o = 1; o < 16; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  const int total = __shfl_sync(0xffffffffu, incl, 8);
+  const int shift = st - (incl - len);  // row's source position minus its concatenated offset
+  int roff[9];
+#pragma unroll
+  for (int r = 1; r < 9; ++r) roff[r] = __shfl_sync(0xffffffffu, incl - len, r);
+
+  int T = 0;
+  u64 best = ~0ull;
+  for (int base = 0; base < total; base += 32) {
+    const int i = base + lane;
+    int row = 0;
+#pragma unroll
+    for (int r = 1; r < 9; ++r) row += i >= roff[r] ? 1 : 0;
+    const int src = i + __shfl_sync(0xffffffffu, shift, row);
+    bool in = false;
+    u64 key = 0;
+    if (i < total) {
+      const float4 c = pts[src];
+      const float d2 = ref_d2(qx, qy, qz, c.x, c.y, c.z);
+      in = d2 < r2;
+      key = make_key(d2, __float_as_int(c.w));
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, in);
+    if (in) {
+      const int pos = T + __popc(m & lt);
+      if (pos < kCandCap) s_cand[pos] = key;
+      best = key < best ? key : best;
+    }
+    T += __popc(m);
+  }
   __syncwarp();
-  const int qm = query_mask[gq];
-  int* io = idx + (size_t)gq * K;
-  int* mo = idx_mask ? idx_mask + (size_t)gq * K : nullptr;
-  int* no = ncount ? ncount + gq : nullptr;
-  int* cc = csr_cnt ? csr_cnt + (size_t)b * N : nullptr;
-  int* cr = csr_rank ? csr_rank + (size_t)gq * K : nullptr;
+  const u64* list = s_cand;
+  int cnt = T;
   if (T > kCandCap) {
     // neighbourhood does not fit on chip: exact index-order scan straight from global memory (rare)
     const float* sx = support_xyz + (size_t)b * N * 3;
-    int cnt = brute_force_collect(
+    cnt = brute_force_collect(
         [&](int i, float& x, float& y, float& z) {
           x = sx[i * 3 + 0];
           y = sx[i * 3 + 1];
           z = sx[i * 3 + 2];
         },
         p.n_valid, qx, qy, qz, r2, cap3k, s_keep);
-    emit_query(s_keep, cnt, s_sorted, K, qm, io, mo, no, cc, cr, csr_all);
-    return;
-  }
-  if (T <= cap3k) {
-    emit_query(s_cand, T, s_sorted, K, qm, io, mo, no, cc, cr, csr_all);
-    return;
-  }
-  // more than 3K candidates: the reference keeps the 3K SMALLEST INDICES (it scans in index order, :64-68),
-  // then overwrites the last kept one with the global nearest if that lies beyond it (:72-75).
-  best = warp_min_u64(best);
-  int kept = 0;  // warp-uniform running count
-  for (int base = 0; base < T; base += 32) {
-    const int i = base + lane;
-    bool keep = false;
-    u64 my = 0;
-    if (i < T) {
-      my = s_cand[i];
-      const unsigned myidx = (unsigned)(my & 0xffffffffu);
-      int r = 0;
-      for (int j = 0; j < T; ++j) r += ((unsigned)(s_cand[j] & 0xffffffffu) < myidx) ? 1 : 0;
-      keep = r < cap3k;
-      if (r == cap3k - 1 && (unsigned)(best & 0xffffffffu) > myidx) my = best;  // overwrite rule
+    list = s_keep;
+  } else if (T > cap3k) {
+    // more than 3K candidates: the reference keeps the 3K SMALLEST INDICES (it scans in index order, :64-68),
+    // then overwrites the last kept one with the global nearest if that lies beyond it (:72-75).
+    best = warp_min_u64(best);
+    int kept = 0;  // warp-uniform running count
+    for (int base = 0; base < T; base += 32) {
+      const int i = base + lane;
+      bool keep = false;
+      u64 my = 0;
+      if (i < T) {
+        my = s_cand[i];
+        const unsigned myidx = (unsigned)(my & 0xffffffffu);
+        int r = 0;
+        for (int j = 0; j < T; ++j) r += ((unsigned)(s_cand[j] & 0xffffffffu) < myidx) ? 1 : 0;
+        keep = r < cap3k;
+        if (r == cap3k - 1 && (unsigned)(best & 0xffffffffu) > myidx) my = best;  // overwrite rule
+      }
+      const unsigned m = __ballot_sync(0xffffffffu, keep);
+      if (keep) s_keep[kept + __popc(m & lt)] = my;
+      kept += __popc(m);
     }
-    const unsigned m = __ballot_sync(0xffffffffu, keep);
-    if (keep) s_keep[kept + __popc(m & lt)] = my;
-    kept += __popc(m);
+    __syncwarp();
+    list = s_keep;
+    cnt = cap3k;
   }
-  __syncwarp();
-  emit_query(s_keep, cap3k, s_sorted, K, qm, io, mo, no, cc, cr, csr_all);
+  emit_query(list, cnt, s_sorted, K, query_mask[gq], idx + gq * K, idx_mask ? idx_mask + gq * K : nullptr,
+             ncount ? ncount + gq : nullptr, csr_cnt ? csr_cnt + (size_t)b * N : nullptr,
+             csr_rank ? csr_rank + gq * K : nullptr, csr_all);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1112,9 +1111,11 @@ static int ball_query_impl(const float* query_xyz, const float* support_xyz, con
   if (first_call_on_device(attr_grid))
     cudaFuncSetAttribute(ball_query_grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
   const long long total = (long long)B * M;
+  // the same points and mask as query and support (every non-strided layer): walk the queries in cell order
+  const int cell_order = query_xyz == support_xyz && query_mask == support_mask && M == N;
   ball_query_grid_kernel<<<(unsigned)((total + kBQWarps - 1) / kBQWarps), kBQWarps * 32, smem, stream>>>(
-      query_xyz, support_xyz, query_mask, params, cell_start, sorted, B, N, M, radius, K, cap, idx, idx_mask, ncount,
-      csr_cnt, csr_rank, csr_all); CL3D_LAUNCHED(1);
+      query_xyz, support_xyz, query_mask, params, cell_start, sorted, B, N, M, radius, K, cap, cell_order, idx,
+      idx_mask, ncount, csr_cnt, csr_rank, csr_all); CL3D_LAUNCHED(1);
   return check_launch("ball_query_grid_kernel");
 }
 
