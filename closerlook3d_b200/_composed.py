@@ -3,9 +3,21 @@ gaussian influence, ...; the max reduction of PosPool / AdaptiveWeight is fused,
 (/root/reference/pytorch/models/local_aggregation_operators.py), built from this package's materialising
 kernels (MaskedQueryAndGroup -> cl3d_ball_query + cl3d_group_points) and torch library ops on the GPU.
 It exists so that every configuration the reference accepts runs here too; it is not the hot path.
+16-bit features are widened to fp32 and the result is rounded back to their dtype (autocast off throughout), like
+the fused operators.
 """
+import functools
+
 import torch
 import torch.nn.functional as F
+
+
+def _fp32(fn):
+    @functools.wraps(fn)
+    def call(m, q_xyz, s_xyz, q_mask, s_mask, feats):
+        with torch.autocast("cuda", enabled=False):
+            return fn(m, q_xyz, s_xyz, q_mask, s_mask, feats.float()).to(feats.dtype)
+    return call
 
 
 def _reduce(agg, idx_mask, query_mask, reduction):
@@ -23,6 +35,7 @@ def _out(module, out):
     return module.out_conv(out) if module.output_conv else module.out_transform(out)
 
 
+@_fp32
 def pospool(m, q_xyz, s_xyz, q_mask, s_mask, feats):
     B, C, M, K = feats.shape[0], feats.shape[1], q_xyz.shape[1], m.nsample
     gf, dp, idx_mask = m.grouper(q_xyz, s_xyz, q_mask, s_mask, feats)
@@ -38,6 +51,7 @@ def pospool(m, q_xyz, s_xyz, q_mask, s_mask, feats):
     return _out(m, _reduce(agg, idx_mask, q_mask, m.reduction))
 
 
+@_fp32
 def adaptive_weight(m, q_xyz, s_xyz, q_mask, s_mask, feats):
     B, C, M, K, S = feats.shape[0], feats.shape[1], q_xyz.shape[1], m.nsample, m.shared_channels
     gf, dp, idx_mask = m.grouper(q_xyz, s_xyz, q_mask, s_mask, feats)
@@ -46,6 +60,7 @@ def adaptive_weight(m, q_xyz, s_xyz, q_mask, s_mask, feats):
     return _out(m, _reduce(agg, idx_mask, q_mask, m.reduction))
 
 
+@_fp32
 def pointwise_mlp(m, q_xyz, s_xyz, q_mask, s_mask, feats):
     gf, dp, idx_mask = m.grouper(q_xyz, s_xyz, q_mask, s_mask, feats)
     center = gf[..., 0:1].expand(-1, -1, -1, m.nsample)
@@ -55,6 +70,7 @@ def pointwise_mlp(m, q_xyz, s_xyz, q_mask, s_mask, feats):
     return _reduce(x, idx_mask, q_mask, m.reduction)
 
 
+@_fp32
 def pseudo_grid(m, q_xyz, s_xyz, q_mask, s_mask, feats):
     B, C, M, K = feats.shape[0], feats.shape[1], q_xyz.shape[1], m.nsample
     gf, dp, idx_mask = m.grouper(q_xyz, s_xyz, q_mask, s_mask, feats)

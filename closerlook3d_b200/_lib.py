@@ -61,6 +61,19 @@ SIGNATURES = {
     "cl3d_pwmlp_fwd_out": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "cl3d_pwmlp_bwd_scratch_floats": (_sz, [_i, _i, _i, _i]),
     "cl3d_pwmlp_bwd": (_i, [_vp] * 16 + [_i, _i, _i, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "cl3d_to_point_major_dt": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
+    "cl3d_to_channel_major_dt": (_i, [_vp, _i, _i, _i, _vp, _i, _vp]),
+    "cl3d_group_points_dt": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "cl3d_group_points_grad_dt": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "cl3d_gather_max_fwd_dt": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp]),
+    "cl3d_gather_max_bwd_dt": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "cl3d_agg_bwd_dt": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _i, _i,
+                             _f, _i, _vp, _i, _vp, _vp, _vp]),
+    "cl3d_bn_relu_fwd_dt": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp]),
+    "cl3d_bn_relu_bwd_dt": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "cl3d_to_point_major_aug_dt": (_i, [_vp, _i, _vp, _i, _i, _i, _f, _vp, _vp]),
+    "cl3d_pwmlp_fwd_out_dt": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp]),
+    "cl3d_pwmlp_bwd_dt": (_i, [_vp, _i] + [_vp] * 15 + [_i, _i, _i, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "cl3d_mhead_save_floats": (_sz, [_i, _i]),
     "cl3d_mhead_fwd_workspace_bytes": (_sz, [_vp, _i, _i]),
     "cl3d_mhead_bwd_workspace_bytes": (_sz, [_vp, _i, _i]),

@@ -339,7 +339,7 @@ __host__ __device__ inline size_t pg_bwd_extra_floats(int CI) {
   return (size_t)kMaxKP * 32 * CI /*wk*/ + (size_t)kAggWarps * kMaxKP * 32 * CI /*per-warp pacc*/;
 }
 
-template <int FAM, int CI>
+template <int FAM, int CI, typename TO>
 __global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID || CI > 3) ? 2 : 3) agg_bwd_kernel(const AggArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -468,7 +468,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID ||
     for (int cl = warp; cl < 32 * CI; cl += kAggWarps) {
       const int c = c0 + cl;
       if (c >= a.C) break;
-      if (j < a.N) a.out[((size_t)b * a.C + c) * a.N + j] = s_out[(size_t)cl * (kTile + 1) + lane];
+      if (j < a.N) store_out<TO>(s_out[(size_t)cl * (kTile + 1) + lane], a, ((size_t)b * a.C + c) * a.N + j);
     }
     __syncthreads();
   }
@@ -752,7 +752,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, 3) sincos_fwd_kernel(const Agg
   }
 }
 
-template <int PI>
+template <int PI, typename TO>
 __global__ void __launch_bounds__(kAggWarps * 32, 3) sincos_bwd_kernel(const AggArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -812,7 +812,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, 3) sincos_bwd_kernel(const Agg
     for (int r = warp; r < 2 * 32 * PI; r += kAggWarps) {
       const int c = pair_row_channel(r, p0, 32 * PI, F);
       if (c < 0) continue;
-      if (j < a.N) a.out[((size_t)b * a.C + c) * a.N + j] = s_out[(size_t)r * (kTile + 1) + lane];
+      if (j < a.N) store_out<TO>(s_out[(size_t)r * (kTile + 1) + lane], a, ((size_t)b * a.C + c) * a.N + j);
     }
     __syncthreads();
   }
@@ -840,12 +840,15 @@ static int launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
   const int ppc = params_per_channel<FAM>(a.nkp);
   const SmemLayout L = smem_layout(32 * CI, ppc * 32 * CI);
   const size_t smem = L.total + (FAM == CL3D_FAM_PSEUDOGRID ? pg_bwd_extra_floats(CI) * sizeof(float) : 0);
-  static std::atomic<unsigned long long> seen{0};
-  allow_big_smem(agg_bwd_kernel<FAM, CI>, seen);
   dim3 grid(grid_x, nchunks);
-  agg_bwd_kernel<FAM, CI><<<grid, kAggWarps * 32, smem, stream>>>(a);
-  CL3D_LAUNCHED(1);
-  return check_launch("agg_bwd_kernel");
+  return with_dtype(a.out_dtype, [&](auto t) {
+    using TO = typename decltype(t)::type;
+    static std::atomic<unsigned long long> seen{0};
+    allow_big_smem(agg_bwd_kernel<FAM, CI, TO>, seen);
+    agg_bwd_kernel<FAM, CI, TO><<<grid, kAggWarps * 32, smem, stream>>>(a);
+    CL3D_LAUNCHED(1);
+    return check_launch("agg_bwd_kernel");
+  });
 }
 
 static int pick_ci(int family, int Cp) {
@@ -880,9 +883,13 @@ static int launch_sincos(const AggArgs& a, bool bwd, int grid_x, cudaStream_t st
     allow_big_smem(sincos_fwd_kernel<PI>, seen);
     sincos_fwd_kernel<PI><<<grid, kAggWarps * 32, L.total, stream>>>(a);
   } else {
-    static std::atomic<unsigned long long> seen{0};
-    allow_big_smem(sincos_bwd_kernel<PI>, seen);
-    sincos_bwd_kernel<PI><<<grid, kAggWarps * 32, L.total, stream>>>(a);
+    with_dtype(a.out_dtype, [&](auto t) {
+      using TO = typename decltype(t)::type;
+      static std::atomic<unsigned long long> seen{0};
+      allow_big_smem(sincos_bwd_kernel<PI, TO>, seen);
+      sincos_bwd_kernel<PI, TO><<<grid, kAggWarps * 32, L.total, stream>>>(a);
+      return CL3D_OK;
+    });
   }
   CL3D_LAUNCHED(1);
   return check_launch("sincos kernel");
@@ -997,14 +1004,15 @@ extern "C" int cl3d_agg_fwd(int family, int reduction, const float* feat_pm, con
   return dispatch_fwd(family, pick_ci(family, a.Cp), a, (cudaStream_t)stream_);
 }
 
-extern "C" int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const float* feat_pm,
-                            const float* query_xyz, const float* support_xyz, const int* ncount,
-                            const int* csr_off, const int* csr_ent, const float* p0, const float* p1, int B, int N,
-                            int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
-                            int influence, float* grad_feat, float* grad_params_partial,
-                            const unsigned char* arg_pm, cl3d_stream_t stream_) {
+extern "C" int cl3d_agg_bwd_dt(int family, int reduction, const float* g_pm, const float* feat_pm,
+                               const float* query_xyz, const float* support_xyz, const int* ncount,
+                               const int* csr_off, const int* csr_ent, const float* p0, const float* p1, int B, int N,
+                               int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
+                               int influence, void* grad_feat, int dtype, float* grad_params_partial,
+                               const unsigned char* arg_pm, cl3d_stream_t stream_) {
   int rc = check_common(family, reduction, B, N, M, K, C, shared, nkp);
   if (rc) return rc;
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_agg_bwd");
   CL3D_REQUIRE(g_pm && query_xyz && support_xyz && ncount && csr_off && csr_ent && grad_feat,
                "cl3d_agg_bwd: null pointer");
   const bool has_params = family == CL3D_FAM_ADAPTIVE_DP || family == CL3D_FAM_PSEUDOGRID;
@@ -1021,7 +1029,8 @@ extern "C" int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const 
   a.csr_ent = csr_ent;
   a.p0 = p0;
   a.p1 = p1;
-  a.out = grad_feat;
+  a.out = static_cast<float*>(grad_feat);
+  a.out_dtype = dtype;
   a.partial = grad_params_partial;
   fill_common(a, B, N, M, K, C, radius, reduction, normalize, shared, nkp, extent, influence);
   a.ntiles = B * ceil_div(N, kTile);
@@ -1032,4 +1041,15 @@ extern "C" int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const 
   if (family == CL3D_FAM_PSEUDOGRID && pg2_supported(a))
     return pg2_launch_bwd(a, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
   return dispatch_bwd(family, pick_ci(family, a.Cp), a, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
+}
+
+extern "C" int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const float* feat_pm,
+                            const float* query_xyz, const float* support_xyz, const int* ncount,
+                            const int* csr_off, const int* csr_ent, const float* p0, const float* p1, int B, int N,
+                            int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
+                            int influence, float* grad_feat, float* grad_params_partial,
+                            const unsigned char* arg_pm, cl3d_stream_t stream_) {
+  return cl3d_agg_bwd_dt(family, reduction, g_pm, feat_pm, query_xyz, support_xyz, ncount, csr_off, csr_ent, p0, p1,
+                         B, N, M, K, C, radius, normalize, shared, nkp, extent, influence, grad_feat, CL3D_DTYPE_F32,
+                         grad_params_partial, arg_pm, stream_);
 }

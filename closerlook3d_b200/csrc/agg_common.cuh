@@ -1,5 +1,7 @@
 // agg_common.cuh -- argument block and tile constants shared by the fused aggregation kernels (agg.cu, pg.cu).
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace cl3d {
@@ -27,8 +29,18 @@ struct AggArgs {
   int reduction, normalize, shared, nkp, influence;
   float inv_radius, extent, inv_extent;
   int ntiles;
+  int out_dtype;              // bwd: CL3D_DTYPE_* of `out` (the backward kernels' TO), fwd: CL3D_DTYPE_F32.  Sits in
+                              // what was padding before arg_pm, so the block's layout and size are unchanged
   unsigned char* arg_pm;      // (B,M,Cp) max reduction only: winning neighbour slot per (query, channel)
 };
+
+// the channel-major store of the backward kernels: `out` holds elements of type TO (fp32 -> TO rounds once).
+// The value comes first so that it is evaluated before the index, as in the assignment `a.out[i] = v`.
+template <typename TO>
+__device__ __forceinline__ void store_out(float v, const AggArgs& a, size_t i) {
+  if constexpr (std::is_same<TO, float>::value) a.out[i] = v;
+  else store_f32(reinterpret_cast<TO*>(a.out) + i, v);
+}
 
 
 // ---------------------------------------------------------------------------------------------

@@ -102,7 +102,7 @@ __global__ void __launch_bounds__(kAggWarps * 32) aggmax_fwd_kernel(const AggArg
   }
 }
 
-template <int FAM, int CI>
+template <int FAM, int CI, typename TO>
 __global__ void __launch_bounds__(kAggWarps * 32) aggmax_bwd_kernel(const AggArgs a) {
   constexpr bool AW = FAM == CL3D_FAM_ADAPTIVE_DP;
   constexpr int NACC = AW ? 4 : 1;
@@ -212,7 +212,7 @@ __global__ void __launch_bounds__(kAggWarps * 32) aggmax_bwd_kernel(const AggArg
     for (int cl = warp; cl < 32 * CI; cl += kAggWarps) {
       const int c = c0 + cl;
       if (c >= a.C) break;
-      if (j < a.N) a.out[((size_t)b * a.C + c) * a.N + j] = s_out[cl][lane];
+      if (j < a.N) store_out<TO>(s_out[cl][lane], a, ((size_t)b * a.C + c) * a.N + j);
     }
     __syncthreads();
   }
@@ -242,7 +242,10 @@ static int launch_max(const AggArgs& a, bool bwd, int grid_x, cudaStream_t strea
   if (!bwd)
     aggmax_fwd_kernel<FAM, CI><<<grid, kAggWarps * 32, 0, stream>>>(a);
   else
-    aggmax_bwd_kernel<FAM, CI><<<grid, kAggWarps * 32, 0, stream>>>(a);
+    with_dtype(a.out_dtype, [&](auto t) {
+      aggmax_bwd_kernel<FAM, CI, typename decltype(t)::type><<<grid, kAggWarps * 32, 0, stream>>>(a);
+      return CL3D_OK;
+    });
   CL3D_LAUNCHED(1);
   return check_launch(bwd ? "aggmax_bwd_kernel" : "aggmax_fwd_kernel");
 }

@@ -6,6 +6,8 @@
 // Batch statistics come from the per-tile partial sums the aggregation kernel already produced, so the
 // forward costs one read + one write of (B,C,M); the backward is two passes (statistics, apply) and writes
 // d(loss)/d(agg) directly in the point-major layout the gather-form aggregation backward consumes.
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace cl3d {
@@ -77,19 +79,20 @@ __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restri
 }
 
 // y = relu((x - mean) * invstd * gamma + beta), channel-major, float4 along M when aligned
+template <typename T>
 __global__ void __launch_bounds__(256) bn_relu_fwd_kernel(const float* __restrict__ x, const float* __restrict__ stats,
                                                           const float* __restrict__ gamma,
                                                           const float* __restrict__ beta, int C, int M,
-                                                          float* __restrict__ y) {
+                                                          T* __restrict__ y) {
   const int row = blockIdx.x;  // b*C + c
   const int c = row % C;
   const float mean = stats[c], invstd = stats[C + c];
   const float sc = invstd * gamma[c], sh = beta[c];
   const float* xr = x + (size_t)row * M;
-  float* yr = y + (size_t)row * M;
+  T* yr = y + (size_t)row * M;
   for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < M; i += gridDim.y * blockDim.x) {
     const float v = __fmaf_rn(__fsub_rn(xr[i], mean), sc, sh);  // the backward recomputes exactly this
-    yr[i] = v > 0.f ? v : 0.f;
+    store_f32(yr + i, v > 0.f ? v : 0.f);
   }
 }
 
@@ -98,18 +101,21 @@ __global__ void __launch_bounds__(256) bn_relu_fwd_kernel(const float* __restric
 constexpr int kBwdTile = 128;
 constexpr int kBwdCh = 32;  // channels staged per shared-memory transpose round in the apply pass
 
-__device__ __forceinline__ void load4(const float* __restrict__ p, int q, int M, bool vec, float (&v)[4]) {
-  if (vec && q + 3 < M) {
+// 16-bit rows (grad_y) are read element by element: they are only 2-byte aligned when M is odd
+template <typename T>
+__device__ __forceinline__ void load4(const T* __restrict__ p, int q, int M, bool vec, float (&v)[4]) {
+  if (std::is_same<T, float>::value && vec && q + 3 < M) {
     const float4 t = *reinterpret_cast<const float4*>(p + q);
     v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
   } else {
 #pragma unroll
-    for (int t = 0; t < 4; ++t) v[t] = (q + t < M) ? p[q + t] : 0.f;
+    for (int t = 0; t < 4; ++t) v[t] = (q + t < M) ? load_f32(p + q + t) : 0.f;
   }
 }
 
 // pass 1: per tile and channel: sum(gy), sum(gy * xhat)
-__global__ void __launch_bounds__(256) bn_relu_bwd_stats_kernel(const float* __restrict__ grad_y,
+template <typename T>
+__global__ void __launch_bounds__(256) bn_relu_bwd_stats_kernel(const T* __restrict__ grad_y,
                                                                 const float* __restrict__ x,
                                                                 const float* __restrict__ stats,
                                                                 const float* __restrict__ gamma,
@@ -147,7 +153,8 @@ __global__ void __launch_bounds__(256) bn_relu_bwd_stats_kernel(const float* __r
 
 // pass 2: g = gamma*invstd*(gy - mean(gy) - xhat*mean(gy*xhat)) (training) or gamma*invstd*gy (eval), written
 // point-major (B,M,Cp) through a shared-memory transpose, kBwdCh channels per round; padding channels = 0.
-__global__ void __launch_bounds__(256) bn_relu_bwd_apply_kernel(const float* __restrict__ grad_y,
+template <typename T>
+__global__ void __launch_bounds__(256) bn_relu_bwd_apply_kernel(const T* __restrict__ grad_y,
                                                                 const float* __restrict__ x,
                                                                 const float* __restrict__ stats,
                                                                 const float* __restrict__ gamma,
@@ -253,30 +260,52 @@ extern "C" int cl3d_bn_finalize(const float* bn_partial, int ntiles, int C, long
   return check_launch("bn_finalize_kernel");
 }
 
-extern "C" int cl3d_bn_relu_fwd(const float* x, const float* save_stats, const float* gamma, const float* beta, int B,
-                                int C, int M, float* y, cl3d_stream_t stream_) {
+extern "C" int cl3d_bn_relu_fwd_dt(const float* x, const float* save_stats, const float* gamma, const float* beta,
+                                   int B, int C, int M, void* y, int dtype, cl3d_stream_t stream_) {
   CL3D_REQUIRE(x && save_stats && gamma && beta && y && B >= 0 && C >= 1 && M >= 1, "cl3d_bn_relu_fwd: bad arguments");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_bn_relu_fwd");
   if (B == 0) return CL3D_OK;
   int chunks = ceil_div(M, 1024);
   chunks = chunks < 1 ? 1 : (chunks > 65535 ? 65535 : chunks);
   dim3 grid(B * C, chunks);
-  bn_relu_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream_>>>(x, save_stats, gamma, beta, C, M, y); CL3D_LAUNCHED(1);
-  return check_launch("bn_relu_fwd_kernel");
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    bn_relu_fwd_kernel<T><<<grid, 256, 0, (cudaStream_t)stream_>>>(x, save_stats, gamma, beta, C, M, static_cast<T*>(y));
+    CL3D_LAUNCHED(1);
+    return check_launch("bn_relu_fwd_kernel");
+  });
+}
+
+extern "C" int cl3d_bn_relu_fwd(const float* x, const float* save_stats, const float* gamma, const float* beta, int B,
+                                int C, int M, float* y, cl3d_stream_t stream_) {
+  return cl3d_bn_relu_fwd_dt(x, save_stats, gamma, beta, B, C, M, y, CL3D_DTYPE_F32, stream_);
+}
+
+extern "C" int cl3d_bn_relu_bwd_dt(const void* grad_y, int dtype, const float* x, const float* save_stats,
+                                   const float* gamma, const float* beta, int B, int C, int M, int training,
+                                   float* partial, float* dgamma_dbeta, float* g_pm, cl3d_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  CL3D_REQUIRE(grad_y && x && save_stats && gamma && beta && partial && dgamma_dbeta && g_pm,
+               "cl3d_bn_relu_bwd: null pointer");
+  CL3D_REQUIRE(B >= 0 && C >= 1 && M >= 1, "cl3d_bn_relu_bwd: bad sizes");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_bn_relu_bwd");
+  if (B == 0) return CL3D_OK;
+  const int ntiles = B * ceil_div(M, kBwdTile);  // <= cl3d_agg_num_tiles(B, M): the caller's partial buffer fits
+  const int Cp = padded_channels(C);
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    const T* gy = static_cast<const T*>(grad_y);
+    bn_relu_bwd_stats_kernel<T><<<ntiles, 256, 0, stream>>>(gy, x, save_stats, gamma, beta, C, M, partial); CL3D_LAUNCHED(1);
+    bn_reduce2_kernel<<<ceil_div(C, 32), 1024, 0, stream>>>(partial, ntiles, C, dgamma_dbeta); CL3D_LAUNCHED(1);
+    bn_relu_bwd_apply_kernel<T><<<ntiles, 256, 0, stream>>>(gy, x, save_stats, gamma, beta, dgamma_dbeta, C, Cp, M,
+                                                            1.0f / (float)((long long)B * M), training, g_pm); CL3D_LAUNCHED(1);
+    return check_launch("bn_relu_bwd kernels");
+  });
 }
 
 extern "C" int cl3d_bn_relu_bwd(const float* grad_y, const float* x, const float* save_stats, const float* gamma,
                                 const float* beta, int B, int C, int M, int training, float* partial,
                                 float* dgamma_dbeta, float* g_pm, cl3d_stream_t stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
-  CL3D_REQUIRE(grad_y && x && save_stats && gamma && beta && partial && dgamma_dbeta && g_pm,
-               "cl3d_bn_relu_bwd: null pointer");
-  CL3D_REQUIRE(B >= 0 && C >= 1 && M >= 1, "cl3d_bn_relu_bwd: bad sizes");
-  if (B == 0) return CL3D_OK;
-  const int ntiles = B * ceil_div(M, kBwdTile);  // <= cl3d_agg_num_tiles(B, M): the caller's partial buffer fits
-  const int Cp = padded_channels(C);
-  bn_relu_bwd_stats_kernel<<<ntiles, 256, 0, stream>>>(grad_y, x, save_stats, gamma, beta, C, M, partial); CL3D_LAUNCHED(1);
-  bn_reduce2_kernel<<<ceil_div(C, 32), 1024, 0, stream>>>(partial, ntiles, C, dgamma_dbeta); CL3D_LAUNCHED(1);
-  bn_relu_bwd_apply_kernel<<<ntiles, 256, 0, stream>>>(grad_y, x, save_stats, gamma, beta, dgamma_dbeta, C, Cp, M,
-                                                       1.0f / (float)((long long)B * M), training, g_pm); CL3D_LAUNCHED(1);
-  return check_launch("bn_relu_bwd kernels");
+  return cl3d_bn_relu_bwd_dt(grad_y, CL3D_DTYPE_F32, x, save_stats, gamma, beta, B, C, M, training, partial,
+                             dgamma_dbeta, g_pm, stream_);
 }

@@ -1,6 +1,8 @@
 // common.cuh -- shared device/host helpers for libcl3d (sm_90a only).
 #pragma once
 #include <atomic>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -52,6 +54,35 @@ inline void allow_big_smem(K kernel, std::atomic<unsigned long long>& seen) {
       cudaGetLastError();  // reported by the launch that follows if the kernel really needs it
   }
 }
+// ---------------------------------------------------------------------------------------------
+// element type of a channel-major tensor at the layout boundary (CL3D_DTYPE_*).  Everything inside stays fp32:
+// a 16-bit value is widened exactly on load, an fp32 result is rounded once (to nearest even) on store.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float load_f32(const float* p) { return *p; }
+__device__ __forceinline__ float load_f32(const __half* p) { return __half2float(*p); }
+__device__ __forceinline__ float load_f32(const __nv_bfloat16* p) { return __bfloat162float(*p); }
+__device__ __forceinline__ void store_f32(float* p, float v) { *p = v; }
+__device__ __forceinline__ void store_f32(__half* p, float v) { *p = __float2half_rn(v); }
+__device__ __forceinline__ void store_f32(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+
+inline bool valid_dtype(int dtype) {
+  return dtype == CL3D_DTYPE_F32 || dtype == CL3D_DTYPE_F16 || dtype == CL3D_DTYPE_BF16;
+}
+template <typename T>
+struct TypeTag {
+  using type = T;
+};
+// Calls fn(TypeTag<T>{}) with the element type of `dtype` (checked by the entry point with valid_dtype).
+template <typename F>
+inline int with_dtype(int dtype, F&& fn) {
+  switch (dtype) {
+    case CL3D_DTYPE_F16: return fn(TypeTag<__half>{});
+    case CL3D_DTYPE_BF16: return fn(TypeTag<__nv_bfloat16>{});
+    default: return fn(TypeTag<float>{});
+  }
+}
+#define CL3D_REQUIRE_DTYPE(dt, what) CL3D_REQUIRE(::cl3d::valid_dtype(dt), "%s: unknown dtype code %d", what, dt)
+
 __host__ __device__ inline int padded_channels(int C) { return (C + 7) & ~7; }
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }

@@ -4,6 +4,8 @@
 
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace cl3d {
@@ -56,7 +58,8 @@ int persistent_grid_cap() {
 // (B,C,N) channel-major -> (B,N,Cp) point-major, zero padded.  32x32 smem tile transpose; reads are
 // coalesced along N, writes along C.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) to_point_major_kernel(const float* __restrict__ in, int C, int N, int Cp,
+template <typename T>
+__global__ void __launch_bounds__(256) to_point_major_kernel(const T* __restrict__ in, int C, int N, int Cp,
                                                              float* __restrict__ out) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
@@ -67,7 +70,7 @@ __global__ void __launch_bounds__(256) to_point_major_kernel(const float* __rest
 #pragma unroll
   for (int r = ty; r < 32; r += 8) {
     const int c = c0 + r, n = n0 + tx;
-    tile[r][tx] = (c < C && n < N) ? in[(size_t)c * N + n] : 0.f;
+    tile[r][tx] = (c < C && n < N) ? load_f32(in + (size_t)c * N + n) : 0.f;
   }
   __syncthreads();
 #pragma unroll
@@ -77,8 +80,9 @@ __global__ void __launch_bounds__(256) to_point_major_kernel(const float* __rest
   }
 }
 
+template <typename T>
 __global__ void __launch_bounds__(256) to_channel_major_kernel(const float* __restrict__ in, int C, int N, int Cp,
-                                                               float* __restrict__ out) {
+                                                               T* __restrict__ out) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const int n0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
@@ -94,7 +98,7 @@ __global__ void __launch_bounds__(256) to_channel_major_kernel(const float* __re
 #pragma unroll
   for (int r = ty; r < 32; r += 8) {
     const int c = c0 + r, n = n0 + tx;
-    if (c < C && n < N) out[(size_t)c * N + n] = tile[tx][r];
+    if (c < C && n < N) store_f32(out + (size_t)c * N + n, tile[tx][r]);
   }
 }
 
@@ -103,27 +107,36 @@ __global__ void __launch_bounds__(256) to_channel_major_kernel(const float* __re
 // (:48-69).  One thread per (c, j) row of K outputs; the gradient is computed in gather form over a
 // per-call scan of idx ... kept simple: these are NOT on the fused hot path.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) group_points_kernel(const float* __restrict__ points,
+template <typename T>
+__global__ void __launch_bounds__(256) group_points_kernel(const T* __restrict__ points,
                                                            const int* __restrict__ idx, int C, int N, int M, int K,
-                                                           float* __restrict__ out) {
+                                                           T* __restrict__ out) {
   const int b = blockIdx.z, c = blockIdx.y;
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= (long long)M * K) return;
-  const float* p = points + ((size_t)b * C + c) * N;
+  const T* p = points + ((size_t)b * C + c) * N;
   out[((size_t)b * C + c) * M * K + e] = p[idx[(size_t)b * M * K + e]];
 }
 
 // Deterministic scatter-add: one warp owns one (b, c) row of grad_points and walks all M*K entries in
 // order, accumulating through shared-memory bins would need N floats; instead use fp32 atomics like the
 // reference but on a zero-filled output.  (Order non-determinism matches the reference's own atomicAdd.)
-__global__ void __launch_bounds__(256) group_points_grad_kernel(const float* __restrict__ grad_out,
+template <typename T>
+__global__ void __launch_bounds__(256) group_points_grad_kernel(const T* __restrict__ grad_out,
                                                                 const int* __restrict__ idx, int C, int N, int M,
                                                                 int K, float* __restrict__ grad_points) {
   const int b = blockIdx.z, c = blockIdx.y;
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= (long long)M * K) return;
   float* gp = grad_points + ((size_t)b * C + c) * N;
-  atomicAdd(gp + idx[(size_t)b * M * K + e], grad_out[((size_t)b * C + c) * M * K + e]);
+  atomicAdd(gp + idx[(size_t)b * M * K + e], load_f32(grad_out + ((size_t)b * C + c) * M * K + e));
+}
+
+// the 16-bit group_points gradient: fp32 accumulation buffer -> dtype, one rounding per element
+template <typename T>
+__global__ void __launch_bounds__(256) convert_kernel(const float* __restrict__ in, size_t n, T* __restrict__ out) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    store_f32(out + i, in[i]);
 }
 
 // out[p] = sum_t partial[t][p].  32 parameters x 32 tile-lanes per CTA; every tile-lane sums a fixed
@@ -166,51 +179,99 @@ extern "C" int cl3d_padded_channels(int C) { return padded_channels(C); }
 extern "C" int cl3d_sm_count(void) { return sm_count(); }
 extern "C" long long cl3d_launch_count(void) { return __atomic_load_n(&g_launches, __ATOMIC_RELAXED); }
 
-extern "C" int cl3d_to_point_major(const float* in_cn, int B, int C, int N, float* out_nc, cl3d_stream_t stream_) {
+extern "C" int cl3d_to_point_major_dt(const void* in_cn, int dtype, int B, int C, int N, float* out_nc,
+                                      cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && in_cn && out_nc, "cl3d_to_point_major: bad arguments");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_to_point_major");
   if (B == 0) return CL3D_OK;
   const int Cp = padded_channels(C);
   dim3 grid(ceil_div(N, 32), ceil_div(Cp, 32), B);
-  to_point_major_kernel<<<grid, 256, 0, stream>>>(in_cn, C, N, Cp, out_nc); CL3D_LAUNCHED(1);
-  return check_launch("to_point_major_kernel");
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    to_point_major_kernel<T><<<grid, 256, 0, stream>>>(static_cast<const T*>(in_cn), C, N, Cp, out_nc); CL3D_LAUNCHED(1);
+    return check_launch("to_point_major_kernel");
+  });
 }
 
-extern "C" int cl3d_to_channel_major(const float* in_nc, int B, int C, int N, float* out_cn, cl3d_stream_t stream_) {
+extern "C" int cl3d_to_point_major(const float* in_cn, int B, int C, int N, float* out_nc, cl3d_stream_t stream_) {
+  return cl3d_to_point_major_dt(in_cn, CL3D_DTYPE_F32, B, C, N, out_nc, stream_);
+}
+
+extern "C" int cl3d_to_channel_major_dt(const float* in_nc, int B, int C, int N, void* out_cn, int dtype,
+                                        cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && in_nc && out_cn, "cl3d_to_channel_major: bad arguments");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_to_channel_major");
   if (B == 0) return CL3D_OK;
   const int Cp = padded_channels(C);
   dim3 grid(ceil_div(N, 32), ceil_div(C, 32), B);
-  to_channel_major_kernel<<<grid, 256, 0, stream>>>(in_nc, C, N, Cp, out_cn); CL3D_LAUNCHED(1);
-  return check_launch("to_channel_major_kernel");
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    to_channel_major_kernel<T><<<grid, 256, 0, stream>>>(in_nc, C, N, Cp, static_cast<T*>(out_cn)); CL3D_LAUNCHED(1);
+    return check_launch("to_channel_major_kernel");
+  });
+}
+
+extern "C" int cl3d_to_channel_major(const float* in_nc, int B, int C, int N, float* out_cn, cl3d_stream_t stream_) {
+  return cl3d_to_channel_major_dt(in_nc, B, C, N, out_cn, CL3D_DTYPE_F32, stream_);
+}
+
+extern "C" int cl3d_group_points_dt(const void* points, int dtype, const int* idx, int B, int C, int N, int M, int K,
+                                    void* out, cl3d_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && M >= 0 && K >= 1 && points && idx && out, "cl3d_group_points: bad arguments");
+  CL3D_REQUIRE(C <= 65535 && B <= 65535, "cl3d_group_points: C or B too large");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_group_points");
+  if (B == 0 || M == 0) return CL3D_OK;
+  const long long ents = (long long)M * K;
+  dim3 grid((unsigned)((ents + 255) / 256), C, B);
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    group_points_kernel<T><<<grid, 256, 0, stream>>>(static_cast<const T*>(points), idx, C, N, M, K, static_cast<T*>(out));
+    CL3D_LAUNCHED(1);
+    return check_launch("group_points_kernel");
+  });
 }
 
 extern "C" int cl3d_group_points(const float* points, const int* idx, int B, int C, int N, int M, int K, float* out,
                                  cl3d_stream_t stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
-  CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && M >= 0 && K >= 1 && points && idx && out, "cl3d_group_points: bad arguments");
-  CL3D_REQUIRE(C <= 65535 && B <= 65535, "cl3d_group_points: C or B too large");
-  if (B == 0 || M == 0) return CL3D_OK;
-  const long long ents = (long long)M * K;
-  dim3 grid((unsigned)((ents + 255) / 256), C, B);
-  group_points_kernel<<<grid, 256, 0, stream>>>(points, idx, C, N, M, K, out); CL3D_LAUNCHED(1);
-  return check_launch("group_points_kernel");
+  return cl3d_group_points_dt(points, CL3D_DTYPE_F32, idx, B, C, N, M, K, out, stream_);
 }
 
-extern "C" int cl3d_group_points_grad(const float* grad_out, const int* idx, int B, int C, int N, int M, int K,
-                                      float* grad_points, cl3d_stream_t stream_) {
+extern "C" int cl3d_group_points_grad_dt(const void* grad_out, int dtype, const int* idx, int B, int C, int N, int M,
+                                         int K, void* grad_points, float* acc, cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && M >= 0 && K >= 1 && grad_out && idx && grad_points,
                "cl3d_group_points_grad: bad arguments");
   CL3D_REQUIRE(C <= 65535 && B <= 65535, "cl3d_group_points_grad: C or B too large");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_group_points_grad");
+  CL3D_REQUIRE(dtype == CL3D_DTYPE_F32 || acc, "cl3d_group_points_grad: a 16-bit gradient needs the fp32 buffer acc");
   if (B == 0) return CL3D_OK;
-  cudaMemsetAsync(grad_points, 0, sizeof(float) * (size_t)B * C * N, stream);
-  if (M == 0) return CL3D_OK;
-  const long long ents = (long long)M * K;
-  dim3 grid((unsigned)((ents + 255) / 256), C, B);
-  group_points_grad_kernel<<<grid, 256, 0, stream>>>(grad_out, idx, C, N, M, K, grad_points); CL3D_LAUNCHED(1);
-  return check_launch("group_points_grad_kernel");
+  // no atomics on 16-bit types: a 16-bit gradient is accumulated in fp32 and converted once
+  float* gp = dtype == CL3D_DTYPE_F32 ? static_cast<float*>(grad_points) : acc;
+  const size_t n = (size_t)B * C * N;
+  cudaMemsetAsync(gp, 0, sizeof(float) * n, stream);
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    if (M > 0) {
+      const long long ents = (long long)M * K;
+      dim3 grid((unsigned)((ents + 255) / 256), C, B);
+      group_points_grad_kernel<T><<<grid, 256, 0, stream>>>(static_cast<const T*>(grad_out), idx, C, N, M, K, gp);
+      CL3D_LAUNCHED(1);
+    }
+    if constexpr (!std::is_same<T, float>::value) {
+      const size_t blocks = (n + 255) / 256;
+      convert_kernel<T><<<(unsigned)(blocks < 65535 ? blocks : 65535), 256, 0, stream>>>(gp, n, static_cast<T*>(grad_points));
+      CL3D_LAUNCHED(1);
+    }
+    return check_launch("group_points_grad_kernel");
+  });
+}
+
+extern "C" int cl3d_group_points_grad(const float* grad_out, const int* idx, int B, int C, int N, int M, int K,
+                                      float* grad_points, cl3d_stream_t stream_) {
+  return cl3d_group_points_grad_dt(grad_out, CL3D_DTYPE_F32, idx, B, C, N, M, K, grad_points, nullptr, stream_);
 }
 
 extern "C" int cl3d_reduce_partials(const float* partial, int ntiles, int P, float* out, cl3d_stream_t stream_) {

@@ -75,12 +75,17 @@ __host__ __device__ inline PgSmem pg_smem(int Cp, bool bwd) {
   return L;
 }
 
-// Coordinates of point r from a packed (n,3) array with two requests instead of three: the 12 bytes start 8-byte
-// aligned for even r (8 + 4) and end 8-byte aligned for odd r (4 + 8).  A scattered 4-byte load costs the L1 one
-// wavefront per distinct line and instruction, and these kernels are bound by exactly that.
+// true when the 12 bytes of a point's coordinates start 4 bytes past an 8-byte boundary (then they END on one).  The
+// address decides, not the point's index: a cloud's rows start at b * n * 3 floats, which is only 4-byte aligned for
+// odd b when the cloud size n is odd.
+__device__ __forceinline__ bool xyz_odd(const float* p) { return (reinterpret_cast<uintptr_t>(p) & 4) != 0; }
+
+// Coordinates of point r from a packed (n,3) array with two requests instead of three: 8 + 4 bytes when they start
+// 8-byte aligned, 4 + 8 when they end so.  A scattered 4-byte load costs the L1 one wavefront per distinct line and
+// instruction, and these kernels are bound by exactly that.
 __device__ __forceinline__ void load_xyz(const float* __restrict__ xyz, int r, float& x, float& y, float& z) {
   const float* p = xyz + (size_t)r * 3;
-  if (r & 1) {
+  if (xyz_odd(p)) {
     x = p[0];
     const float2 t = *reinterpret_cast<const float2*>(p + 1);
     y = t.x;
@@ -242,7 +247,7 @@ __device__ __forceinline__ void pg_load_params(const AggArgs& a, const PgSmem& L
 // =================================================================================================
 // (The backward's bound of 3 CTAs per SM sets its register budget; its shared memory -- 88 KB at 72 channels --
 // lets 2 be resident.)
-template <bool BWD, bool CHUNKED>
+template <bool BWD, bool CHUNKED, typename TO>
 __global__ void __launch_bounds__(kPgWarps * 32, BWD ? 3 : 4) pg2_kernel(const AggArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -357,7 +362,7 @@ __global__ void __launch_bounds__(kPgWarps * 32, BWD ? 3 : 4) pg2_kernel(const A
     // ---- tile -> channel-major (B,C,P)
     const int p = p0 + lane;
     for (int c = warp; c < Cv; c += kPgWarps)
-      if (p < P) a.out[((size_t)b * a.C + c0 + c) * P + p] = s_out[(size_t)c * (kPgTile + 1) + lane];
+      if (p < P) store_out<TO>(s_out[(size_t)c * (kPgTile + 1) + lane], a, ((size_t)b * a.C + c0 + c) * P + p);
     if constexpr (!BWD) {
       if (a.partial) {  // BatchNorm partial sums of the tile: the warps' sums in a fixed order
         for (int e = threadIdx.x; e < 2 * Cv; e += blockDim.x) {
@@ -496,7 +501,11 @@ __device__ __forceinline__ Pg3Next pg3_fetch(const AggArgs& a, int tile, int pl,
   if (n.e0 + lane < n.e1) {  // 12 bytes in two requests, the 8-byte piece 8-byte aligned at both ends (as load_xyz)
     const float* q = (BWD ? a.query_xyz : a.support_xyz) + ((size_t)b * R + n.r) * 3;
     const uint32_t d = h_a + (uint32_t)(lane * kPg3HRow + kPg3NbrW + (n.r & 1)) * 4;
-    if (n.r & 1) {
+    if (xyz_odd(q) != (bool)(n.r & 1)) {  // odd cloud size, odd b: the source's alignment differs from the slot's
+      cp_async4(d, q);
+      cp_async4(d + 4, q + 1);
+      cp_async4(d + 8, q + 2);
+    } else if (n.r & 1) {
       cp_async4(d, q);
       cp_async8(d + 4, q + 1);
     } else {
@@ -611,7 +620,7 @@ __device__ __forceinline__ int pg3_sum_index(int lane, int j) {
 //              BatchNorm partial row (sum, sum of squares over the tile's 32 queries) per tile.
 // BWD = true : centre = support point j, rows = g_pm[q_e] over the transposed list of j; out[b,:,j] = d/df and
 //              d/dWk in registers -> one partial row per CTA.
-template <bool BWD, int NT>
+template <bool BWD, int NT, typename TO>
 __device__ __forceinline__ void pg3_body(const AggArgs& a, int partial_rows) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -755,7 +764,11 @@ __device__ __forceinline__ void pg3_body(const AggArgs& a, int partial_rows) {
     // ---- tile -> channel-major (B,C,P)
     const int p = p0 + lane;
     for (int c = warp; c < Cv; c += kPgWarps)
-      if (p < P) a.out[((size_t)b * a.C + c0 + c) * P + p] = s_out[(size_t)c * (kPgTile + 1) + lane];
+      if (p < P) {
+        // fp32: the plain assignment (through store_out the compiler schedules this kernel's loops differently)
+        if constexpr (std::is_same<TO, float>::value) a.out[((size_t)b * a.C + c0 + c) * P + p] = s_out[(size_t)c * (kPgTile + 1) + lane];
+        else store_out<TO>(s_out[(size_t)c * (kPgTile + 1) + lane], a, ((size_t)b * a.C + c0 + c) * P + p);
+      }
     if constexpr (!BWD) {
       if (a.partial) {  // BatchNorm partial sums of the tile, over its 32 queries in order (absent ones hold 0)
         for (int e = threadIdx.x; e < 2 * Cv; e += blockDim.x) {
@@ -796,11 +809,11 @@ __device__ __forceinline__ void pg3_body(const AggArgs& a, int partial_rows) {
 
 template <int NT>
 __global__ void __launch_bounds__(kPgWarps * 32, kPg3CtasPerSM) pg3_fwd_kernel(const AggArgs a) {
-  pg3_body<false, NT>(a, 0);
+  pg3_body<false, NT, float>(a, 0);
 }
-template <int NT>
+template <int NT, typename TO>
 __global__ void __launch_bounds__(kPgWarps * 32, kPg3CtasPerSM) pg3_bwd_kernel(const AggArgs a, int partial_rows) {
-  pg3_body<true, NT>(a, partial_rows);
+  pg3_body<true, NT, TO>(a, partial_rows);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -822,11 +835,16 @@ bool pg3_fwd_supported(const AggArgs& a) { return a.Cp <= kPg3FwdMaxCp && pg3_su
 
 template <bool BWD, int NT>
 static void pg3_launch_nt(const AggArgs& a, dim3 grid, int partial_rows, cudaStream_t stream) {
-  static std::atomic<unsigned long long> seen{0};
   if constexpr (BWD) {
-    allow_big_smem(pg3_bwd_kernel<NT>, seen);
-    pg3_bwd_kernel<NT><<<grid, kPgWarps * 32, pg3_smem(true).total, stream>>>(a, partial_rows);
+    with_dtype(a.out_dtype, [&](auto t) {
+      using TO = typename decltype(t)::type;
+      static std::atomic<unsigned long long> seen_b{0};
+      allow_big_smem(pg3_bwd_kernel<NT, TO>, seen_b);
+      pg3_bwd_kernel<NT, TO><<<grid, kPgWarps * 32, pg3_smem(true).total, stream>>>(a, partial_rows);
+      return CL3D_OK;
+    });
   } else {
+    static std::atomic<unsigned long long> seen{0};
     allow_big_smem(pg3_fwd_kernel<NT>, seen);
     pg3_fwd_kernel<NT><<<grid, kPgWarps * 32, pg3_smem(false).total, stream>>>(a);
   }
@@ -877,12 +895,12 @@ int pg2_launch_fwd(const AggArgs& a, cudaStream_t stream) {
   const PgSmem L = pg_smem(pg_chunk_width(a.Cp, nchunks), false);
   static std::atomic<unsigned long long> seen{0};
   if (nchunks == 1) {
-    allow_big_smem(pg2_kernel<false, false>, seen);
-    pg2_kernel<false, false><<<a.ntiles, kPgWarps * 32, L.total, stream>>>(a);
+    allow_big_smem(pg2_kernel<false, false, float>, seen);
+    pg2_kernel<false, false, float><<<a.ntiles, kPgWarps * 32, L.total, stream>>>(a);
   } else {
     static std::atomic<unsigned long long> seen_c{0};
-    allow_big_smem(pg2_kernel<false, true>, seen_c);
-    pg2_kernel<false, true><<<dim3(a.ntiles, nchunks), kPgWarps * 32, L.total, stream>>>(a);
+    allow_big_smem(pg2_kernel<false, true, float>, seen_c);
+    pg2_kernel<false, true, float><<<dim3(a.ntiles, nchunks), kPgWarps * 32, L.total, stream>>>(a);
   }
   CL3D_LAUNCHED(1);
   return check_launch("pg2_kernel<fwd>");
@@ -893,15 +911,19 @@ int pg2_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
 
   const int nchunks = pg_num_chunks(a.Cp);
   const PgSmem L = pg_smem(pg_chunk_width(a.Cp, nchunks), true);
-  static std::atomic<unsigned long long> seen{0};
-  if (nchunks == 1) {
-    allow_big_smem(pg2_kernel<true, false>, seen);
-    pg2_kernel<true, false><<<grid_x, kPgWarps * 32, L.total, stream>>>(a);
-  } else {
-    static std::atomic<unsigned long long> seen_c{0};
-    allow_big_smem(pg2_kernel<true, true>, seen_c);
-    pg2_kernel<true, true><<<dim3(grid_x, nchunks), kPgWarps * 32, L.total, stream>>>(a);
-  }
+  with_dtype(a.out_dtype, [&](auto t) {
+    using TO = typename decltype(t)::type;
+    static std::atomic<unsigned long long> seen{0};
+    if (nchunks == 1) {
+      allow_big_smem(pg2_kernel<true, false, TO>, seen);
+      pg2_kernel<true, false, TO><<<grid_x, kPgWarps * 32, L.total, stream>>>(a);
+    } else {
+      static std::atomic<unsigned long long> seen_c{0};
+      allow_big_smem(pg2_kernel<true, true, TO>, seen_c);
+      pg2_kernel<true, true, TO><<<dim3(grid_x, nchunks), kPgWarps * 32, L.total, stream>>>(a);
+    }
+    return CL3D_OK;
+  });
   CL3D_LAUNCHED(1);
   return check_launch("pg2_kernel<bwd>");
 }

@@ -15,10 +15,10 @@ constexpr int kPoolWarps = 8;
 constexpr int kPoolTile = 32;
 constexpr int kPoolU = 4;
 
-template <int CI>
+template <int CI, typename T>
 __global__ void __launch_bounds__(kPoolWarps * 32) gather_max_fwd_kernel(const float* __restrict__ feat_pm,
                                                                          const int* __restrict__ idx, int N, int M,
-                                                                         int K, int C, int Cp, float* __restrict__ out,
+                                                                         int K, int C, int Cp, T* __restrict__ out,
                                                                          unsigned char* __restrict__ arg) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -81,12 +81,13 @@ __global__ void __launch_bounds__(kPoolWarps * 32) gather_max_fwd_kernel(const f
   for (int cl = warp; cl < 32 * CI; cl += kPoolWarps) {
     const int c = c0 + cl;
     if (c >= C) break;
-    if (q < M) out[((size_t)b * C + c) * M + q] = s_out[(size_t)cl * (kPoolTile + 1) + lane];
+    if (q < M) store_f32(out + ((size_t)b * C + c) * M + q, s_out[(size_t)cl * (kPoolTile + 1) + lane]);
   }
 }
 
 // grad_pm[b, idx[b,q,arg[b,q,c]], c] += grad_out[b,c,q]
-__global__ void __launch_bounds__(256) gather_max_bwd_kernel(const float* __restrict__ grad_out,
+template <typename T>
+__global__ void __launch_bounds__(256) gather_max_bwd_kernel(const T* __restrict__ grad_out,
                                                              const int* __restrict__ idx,
                                                              const unsigned char* __restrict__ arg, int N, int M, int K,
                                                              int C, int Cp, float* __restrict__ grad_pm) {
@@ -97,7 +98,7 @@ __global__ void __launch_bounds__(256) gather_max_bwd_kernel(const float* __rest
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int c = warp; c < C; c += 8) {
     const int q = q0 + lane;
-    s_g[(size_t)lane * (C + 1) + c] = q < M ? grad_out[((size_t)b * C + c) * M + q] : 0.f;
+    s_g[(size_t)lane * (C + 1) + c] = q < M ? load_f32(grad_out + ((size_t)b * C + c) * M + q) : 0.f;
   }
   __syncthreads();
   for (int ql = warp; ql < 32; ql += 8) {
@@ -111,14 +112,14 @@ __global__ void __launch_bounds__(256) gather_max_bwd_kernel(const float* __rest
   }
 }
 
-template <int CI>
-static int launch_pool_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, int Cp, float* out,
+template <int CI, typename T>
+static int launch_pool_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, int Cp, T* out,
                            unsigned char* arg, cudaStream_t stream) {
   const size_t smem = align_up((size_t)kPoolWarps * K * 4, 16) + (size_t)32 * CI * (kPoolTile + 1) * 4;
   static std::atomic<unsigned long long> seen{0};
-  allow_big_smem(gather_max_fwd_kernel<CI>, seen);
+  allow_big_smem(gather_max_fwd_kernel<CI, T>, seen);
   dim3 grid(B * ceil_div(M, kPoolTile), ceil_div(Cp, 32 * CI));
-  gather_max_fwd_kernel<CI><<<grid, kPoolWarps * 32, smem, stream>>>(feat_pm, idx, N, M, K, C, Cp, out, arg);
+  gather_max_fwd_kernel<CI, T><<<grid, kPoolWarps * 32, smem, stream>>>(feat_pm, idx, N, M, K, C, Cp, out, arg);
   CL3D_LAUNCHED(1);
   return check_launch("gather_max_fwd_kernel");
 }
@@ -127,35 +128,55 @@ static int launch_pool_fwd(const float* feat_pm, const int* idx, int B, int N, i
 
 using namespace cl3d;
 
-extern "C" int cl3d_gather_max_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, float* out,
-                                   unsigned char* arg, cl3d_stream_t stream_) {
+extern "C" int cl3d_gather_max_fwd_dt(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C,
+                                      void* out, int dtype, unsigned char* arg, cl3d_stream_t stream_) {
   CL3D_REQUIRE(feat_pm && idx && out && arg && B >= 0 && N >= 1 && M >= 1 && K >= 1 && K <= 255 && C >= 1,
                "cl3d_gather_max_fwd: bad arguments (K <= 255)");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_gather_max_fwd");
   if (B == 0) return CL3D_OK;
   const int Cp = padded_channels(C);
   int ci = ceil_div(Cp, 32);
   if (ci > 4) ci = 4;
   cudaStream_t s = (cudaStream_t)stream_;
-  switch (ci) {
-    case 1: return launch_pool_fwd<1>(feat_pm, idx, B, N, M, K, C, Cp, out, arg, s);
-    case 2: return launch_pool_fwd<2>(feat_pm, idx, B, N, M, K, C, Cp, out, arg, s);
-    case 3: return launch_pool_fwd<3>(feat_pm, idx, B, N, M, K, C, Cp, out, arg, s);
-    default: return launch_pool_fwd<4>(feat_pm, idx, B, N, M, K, C, Cp, out, arg, s);
-  }
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    T* o = static_cast<T*>(out);
+    switch (ci) {
+      case 1: return launch_pool_fwd<1>(feat_pm, idx, B, N, M, K, C, Cp, o, arg, s);
+      case 2: return launch_pool_fwd<2>(feat_pm, idx, B, N, M, K, C, Cp, o, arg, s);
+      case 3: return launch_pool_fwd<3>(feat_pm, idx, B, N, M, K, C, Cp, o, arg, s);
+      default: return launch_pool_fwd<4>(feat_pm, idx, B, N, M, K, C, Cp, o, arg, s);
+    }
+  });
 }
 
-extern "C" int cl3d_gather_max_bwd(const float* grad_out, const int* idx, const unsigned char* arg, int B, int N,
-                                   int M, int K, int C, float* grad_pm, cl3d_stream_t stream_) {
+extern "C" int cl3d_gather_max_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, float* out,
+                                   unsigned char* arg, cl3d_stream_t stream_) {
+  return cl3d_gather_max_fwd_dt(feat_pm, idx, B, N, M, K, C, out, CL3D_DTYPE_F32, arg, stream_);
+}
+
+extern "C" int cl3d_gather_max_bwd_dt(const void* grad_out, int dtype, const int* idx, const unsigned char* arg, int B,
+                                      int N, int M, int K, int C, float* grad_pm, cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(grad_out && idx && arg && grad_pm && B >= 0 && N >= 1 && M >= 1 && K >= 1 && C >= 1,
                "cl3d_gather_max_bwd: bad arguments");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_gather_max_bwd");
   if (B == 0) return CL3D_OK;
   const int Cp = padded_channels(C);
   cudaMemsetAsync(grad_pm, 0, sizeof(float) * (size_t)B * N * Cp, stream);
   const size_t smem = (size_t)32 * (C + 1) * sizeof(float);
-  static std::atomic<unsigned long long> seen{0};
-  allow_big_smem(gather_max_bwd_kernel, seen);
-  gather_max_bwd_kernel<<<B * ceil_div(M, 32), 256, smem, stream>>>(grad_out, idx, arg, N, M, K, C, Cp, grad_pm);
-  CL3D_LAUNCHED(1);
-  return check_launch("gather_max_bwd_kernel");
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    static std::atomic<unsigned long long> seen{0};
+    allow_big_smem(gather_max_bwd_kernel<T>, seen);
+    gather_max_bwd_kernel<T><<<B * ceil_div(M, 32), 256, smem, stream>>>(static_cast<const T*>(grad_out), idx, arg, N, M,
+                                                                          K, C, Cp, grad_pm);
+    CL3D_LAUNCHED(1);
+    return check_launch("gather_max_bwd_kernel");
+  });
+}
+
+extern "C" int cl3d_gather_max_bwd(const float* grad_out, const int* idx, const unsigned char* arg, int B, int N,
+                                   int M, int K, int C, float* grad_pm, cl3d_stream_t stream_) {
+  return cl3d_gather_max_bwd_dt(grad_out, CL3D_DTYPE_F32, idx, arg, B, N, M, K, C, grad_pm, stream_);
 }

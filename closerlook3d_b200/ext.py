@@ -3,13 +3,16 @@
 argument order and return shapes, on libcl3d's kernels.  Put it in sys.modules['pt_custom_ops._ext'] to run the
 reference's own `pt_utils.py` / operator modules (unfused) on these kernels."""
 from . import ops
+from ._lib import require_cuda
 
 
 def group_points(points, idx):
+    require_cuda(points, "points", ops.F32)   # fp32 only, as the reference's CHECK_IS_FLOAT
     return ops.group_points(points, idx)
 
 
 def group_points_grad(grad_out, idx, n):
+    require_cuda(grad_out, "grad_out", ops.F32)
     return ops.group_points_grad(grad_out, idx, n)
 
 

@@ -35,7 +35,9 @@ class _FusedAggBNReLU(Function):
     """agg = fused_aggregation(features) ; out = relu(batchnorm1d(agg))"""
 
     @staticmethod
+    @ops.no_autocast
     def forward(ctx, features, p0, p1, bn_weight, bn_bias, spec, nl, query_xyz, support_xyz, bn):
+        # features: fp32, fp16 or bf16; out and d/dfeatures come in that dtype, everything between is fp32
         B, C, N = features.shape
         M = query_xyz.shape[1]
         feat_pm = ops.to_point_major(features)   # overlaps the neighbour search running on the side stream
@@ -68,16 +70,17 @@ class _FusedAggBNReLU(Function):
             if bn.momentum is None:  # cumulative moving average, as nn.BatchNorm1d
                 momentum = 1.0 / float(bn.num_batches_tracked)
         stats = ops.bn_finalize(partial, C, B * M, bn.eps, momentum, training, bn.running_mean, bn.running_var)
-        out = ops.bn_relu_fwd(agg, stats, bn_weight, bn_bias)
+        out = ops.bn_relu_fwd(agg, stats, bn_weight, bn_bias, dtype=features.dtype)
         if any(ctx.needs_input_grad):
             nl.prefetch_csr(all_slots=False)      # transposed lists for the backward, built behind the forward
-        ctx.spec, ctx.nl, ctx.training, ctx.N = spec, nl, training, N
+        ctx.spec, ctx.nl, ctx.training, ctx.N, ctx.dtype = spec, nl, training, N, features.dtype
         needs_feat = spec.family in (ops.FAM_ADAPTIVE_DP, ops.FAM_PSEUDOGRID)
         ctx.save_for_backward(agg, stats, bn_weight, bn_bias, query_xyz, support_xyz, p0, p1,
                               feat_pm if needs_feat else None, arg)
         return out
 
     @staticmethod
+    @ops.no_autocast
     def backward(ctx, grad_out):
         agg, stats, bn_weight, bn_bias, query_xyz, support_xyz, p0, p1, feat_pm, arg = ctx.saved_tensors
         spec, nl = ctx.spec, ctx.nl
@@ -86,7 +89,7 @@ class _FusedAggBNReLU(Function):
         off, ent = nl.csr()
         grad_feat, pg = ops.agg_bwd(spec.family, spec.reduction, g_pm, feat_pm, query_xyz, support_xyz, nl.ncount,
                                     off, ent, p0, p1, C, ctx.N, spec.nsample, spec.radius, spec.normalize,
-                                    spec.shared, spec.nkp, spec.extent, spec.influence, arg=arg)
+                                    spec.shared, spec.nkp, spec.extent, spec.influence, arg=arg, dtype=ctx.dtype)
         gp0 = gp1 = None
         if spec.family == ops.FAM_ADAPTIVE_DP:  # pg: (4, C) rows x,y,z,bias per channel -> fold shared groups
             S = spec.shared
@@ -106,8 +109,8 @@ def _check_inputs(query_xyz, support_xyz, query_mask, support_mask, support_feat
     require_cuda(support_mask, "support_mask", torch.int32)
     if not support_features.is_cuda:
         raise RuntimeError("points must be a CUDA tensor (CPU not supported)")
-    if support_features.dtype != torch.float32:
-        raise RuntimeError("points must be a float tensor")
+    if support_features.dtype not in ops.DTYPE_CODE:
+        raise RuntimeError("points must be a float tensor (float32, float16 or bfloat16)")
 
 
 def _out_block(module, in_channels, out_channels, momentum):
@@ -139,6 +142,7 @@ class PosPool(nn.Module):
         return (not self.output_conv) and self.position_embedding in ("xyz", "sin_cos") and \
             (self.reduction in ("avg", "mean", "sum") or (self.reduction == "max" and self.nsample <= 256))
 
+    @ops.no_autocast
     def forward(self, query_xyz, support_xyz, query_mask, support_mask, support_features):
         """(B,M,3),(B,N,3),(B,M) i32,(B,N) i32,(B,C,N) -> (B,C_out,M)   (reference :47-112)"""
         if self.position_embedding not in ("xyz", "sin_cos"):
@@ -200,6 +204,7 @@ class AdaptiveWeight(nn.Module):
         return (not self.output_conv) and self.num_mlps == 1 and \
             (self.reduction in ("avg", "mean", "sum") or (self.reduction == "max" and self.nsample <= 256))
 
+    @ops.no_autocast
     def forward(self, query_xyz, support_xyz, query_mask, support_mask, support_features):
         """reference :170-224"""
         if self.weight_type != 'dp':
@@ -246,6 +251,7 @@ class PseudoGrid(nn.Module):
     def _fusable(self):
         return (not self.output_conv) and self.KP_influence in ("linear", "constant") and self.num_kernel_points <= 16
 
+    @ops.no_autocast
     def forward(self, query_xyz, support_xyz, query_mask, support_mask, support_features):
         """reference :368-426"""
         if self.KP_influence not in ("constant", "linear", "gaussian"):
@@ -299,6 +305,7 @@ class PointWiseMLP(nn.Module):
     def _fusable(self):
         return self.num_mlps == 1 and self.reduction == "max"
 
+    @ops.no_autocast
     def forward(self, query_xyz, support_xyz, query_mask, support_mask, support_features):
         """reference :274-316"""
         if self.feature_type != 'dp_fi_df':
@@ -329,7 +336,8 @@ class LocalAggregation(nn.Module):
 
     def forward(self, query_xyz, support_xyz, query_mask, support_mask, support_features):
         """query_xyz (B,M,3), support_xyz (B,N,3), masks (B,M)/(B,N) int32, support_features (B,C_in,N)
-        -> (B,C_out,M)   (reference :452-464)"""
+        -> (B,C_out,M)   (reference :452-464).  support_features may be float32, float16 or bfloat16 (e.g. under
+        torch.autocast): the output and the feature gradient come in that dtype, the arithmetic is fp32."""
         if support_features.is_cuda and support_features.device.index != torch.cuda.current_device():
             with torch.cuda.device(support_features.device):  # streams / launches belong to the tensors' device
                 return self.local_aggregation_operator(query_xyz, support_xyz, query_mask, support_mask,

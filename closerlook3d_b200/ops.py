@@ -10,6 +10,21 @@ from ._lib import check, ptr, require_cuda, stream_ptr
 I32 = torch.int32
 F32 = torch.float32
 
+# element type of a channel-major feature tensor -> CL3D_DTYPE_* (include/cl3d.h).  The features set the dtype of
+# every tensor that crosses the layout boundary; everything inside the library stays fp32.
+DTYPE_CODE = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+
+
+def require_features(t, name):
+    """CUDA, contiguous, float32 / float16 / bfloat16 -> the dtype code"""
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor (CPU not supported)")
+    if not t.is_contiguous():
+        raise RuntimeError(f"{name} must be a contiguous tensor")
+    if t.dtype not in DTYPE_CODE:
+        raise RuntimeError(f"{name} must be a float tensor (float32, float16 or bfloat16)")
+    return DTYPE_CODE[t.dtype]
+
 
 def _on_device(fn):
     """Run `fn` with the CUDA device of its tensor arguments current (kernels, the stream passed to the library and
@@ -29,6 +44,18 @@ def _on_device(fn):
         if dev is None or dev.index == torch.cuda.current_device():
             return fn(*args, **kw)
         with torch.cuda.device(dev):
+            return fn(*args, **kw)
+    return call
+
+
+def no_autocast(fn):
+    """Run `fn` with CUDA autocast off.  The library's modules and autograd Functions decide dtypes themselves (the
+    features' dtype at the layout boundary, fp32 inside), so no torch op of theirs may be recast by autocast."""
+    import functools
+
+    @functools.wraps(fn)
+    def call(*args, **kw):
+        with torch.autocast("cuda", enabled=False):
             return fn(*args, **kw)
     return call
 
@@ -128,44 +155,47 @@ def build_csr(idx, ncount, N):
 
 @_on_device
 def to_point_major(x_cn):
-    """(B,C,N) -> (B,N,Cp) zero-padded rows"""
-    require_cuda(x_cn, "features", F32)
+    """(B,C,N) f32 / f16 / bf16 -> (B,N,Cp) fp32 zero-padded rows"""
+    dt = require_features(x_cn, "features")
     B, C, N = x_cn.shape
     out = _empty_pm(B, N, padded_channels(C), x_cn.device)
-    check(_lib.lib().cl3d_to_point_major(ptr(x_cn), B, C, N, ptr(out), stream_ptr()), "cl3d_to_point_major")
+    check(_lib.lib().cl3d_to_point_major_dt(ptr(x_cn), dt, B, C, N, ptr(out), stream_ptr()), "cl3d_to_point_major")
     return out
 
 
 @_on_device
-def to_channel_major(x_nc, C):
-    """(B,N,Cp) -> (B,C,N)"""
+def to_channel_major(x_nc, C, dtype=F32):
+    """(B,N,Cp) fp32 -> (B,C,N) in `dtype`"""
     B, N, Cp = x_nc.shape
     assert Cp == padded_channels(C)
-    out = torch.empty(B, C, N, dtype=F32, device=x_nc.device)
-    check(_lib.lib().cl3d_to_channel_major(ptr(x_nc), B, C, N, ptr(out), stream_ptr()), "cl3d_to_channel_major")
+    out = torch.empty(B, C, N, dtype=dtype, device=x_nc.device)
+    check(_lib.lib().cl3d_to_channel_major_dt(ptr(x_nc), B, C, N, ptr(out), DTYPE_CODE[dtype], stream_ptr()),
+          "cl3d_to_channel_major")
     return out
 
 
 @_on_device
 def group_points(points, idx):
-    require_cuda(points, "points", F32)
+    dt = require_features(points, "points")
     require_cuda(idx, "idx", I32)
     B, C, N = points.shape
     _, M, K = idx.shape
-    out = torch.empty(B, C, M, K, dtype=F32, device=points.device)
-    check(_lib.lib().cl3d_group_points(ptr(points), ptr(idx), B, C, N, M, K, ptr(out), stream_ptr()),
+    out = torch.empty(B, C, M, K, dtype=points.dtype, device=points.device)
+    check(_lib.lib().cl3d_group_points_dt(ptr(points), dt, ptr(idx), B, C, N, M, K, ptr(out), stream_ptr()),
           "cl3d_group_points")
     return out
 
 
 @_on_device
 def group_points_grad(grad_out, idx, n):
-    require_cuda(grad_out, "grad_out", F32)
+    """a 16-bit gradient is accumulated in an fp32 buffer and rounded once"""
+    dt = require_features(grad_out, "grad_out")
     require_cuda(idx, "idx", I32)
     B, C, M, K = grad_out.shape
-    out = torch.empty(B, C, int(n), dtype=F32, device=grad_out.device)
-    check(_lib.lib().cl3d_group_points_grad(ptr(grad_out), ptr(idx), B, C, int(n), M, K, ptr(out), stream_ptr()),
-          "cl3d_group_points_grad")
+    out = torch.empty(B, C, int(n), dtype=grad_out.dtype, device=grad_out.device)
+    acc = torch.empty(B, C, int(n), dtype=F32, device=grad_out.device) if dt else None
+    check(_lib.lib().cl3d_group_points_grad_dt(ptr(grad_out), dt, ptr(idx), B, C, int(n), M, K, ptr(out), ptr(acc),
+                                               stream_ptr()), "cl3d_group_points_grad")
     return out
 
 
@@ -207,21 +237,21 @@ def agg_fwd(family, reduction, feat_pm, query_xyz, support_xyz, idx, ncount, p0,
 
 @_on_device
 def agg_bwd(family, reduction, g_pm, feat_pm, query_xyz, support_xyz, ncount, csr_off, csr_ent, p0, p1, C, N, K,
-            radius, normalize, shared=1, nkp=0, extent=1.0, influence=0, arg=None):
-    """-> (grad_feat (B,C,N), param_grad (P//C, C) | None)   P = 4C (adaptive: x,y,z,bias) or nkp*C;
-    arg = the forward's winning slots (max reduction)"""
+            radius, normalize, shared=1, nkp=0, extent=1.0, influence=0, arg=None, dtype=F32):
+    """-> (grad_feat (B,C,N) in `dtype`, param_grad (P//C, C) fp32 | None)   P = 4C (adaptive: x,y,z,bias) or
+    nkp*C; arg = the forward's winning slots (max reduction)"""
     B, M, Cp = g_pm.shape
     L = _lib.lib()
     dev = g_pm.device
-    grad_feat = torch.empty(B, C, N, dtype=F32, device=dev)
+    grad_feat = torch.empty(B, C, N, dtype=dtype, device=dev)
     P = L.cl3d_agg_num_params(family, C, shared, nkp)
     partial = None
     if P > 0:
         partial = torch.empty(L.cl3d_agg_bwd_num_blocks(B, N), P, dtype=F32, device=dev)
-    check(L.cl3d_agg_bwd(family, reduction, ptr(g_pm), ptr(feat_pm), ptr(query_xyz), ptr(support_xyz), ptr(ncount),
-                         ptr(csr_off), ptr(csr_ent), ptr(p0), ptr(p1), B, N, M, K, C, float(radius), int(normalize),
-                         int(shared), int(nkp), float(extent), int(influence), ptr(grad_feat), ptr(partial),
-                         ptr(arg), stream_ptr()), "cl3d_agg_bwd")
+    check(L.cl3d_agg_bwd_dt(family, reduction, ptr(g_pm), ptr(feat_pm), ptr(query_xyz), ptr(support_xyz), ptr(ncount),
+                            ptr(csr_off), ptr(csr_ent), ptr(p0), ptr(p1), B, N, M, K, C, float(radius), int(normalize),
+                            int(shared), int(nkp), float(extent), int(influence), ptr(grad_feat), DTYPE_CODE[dtype],
+                            ptr(partial), ptr(arg), stream_ptr()), "cl3d_agg_bwd")
     pg = reduce_partials(partial).view(P // C, C) if P > 0 else None
     return grad_feat, pg
 
@@ -239,25 +269,27 @@ def bn_finalize(bn_partial, C, count, eps, momentum, training, running_mean, run
 
 
 @_on_device
-def bn_relu_fwd(x, stats, gamma, beta):
+def bn_relu_fwd(x, stats, gamma, beta, dtype=F32):
+    """x (B,C,M) fp32 -> y in `dtype`"""
     B, C, M = x.shape
-    y = torch.empty_like(x)
-    check(_lib.lib().cl3d_bn_relu_fwd(ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, ptr(y), stream_ptr()),
-          "cl3d_bn_relu_fwd")
+    y = torch.empty(B, C, M, dtype=dtype, device=x.device)
+    check(_lib.lib().cl3d_bn_relu_fwd_dt(ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, ptr(y), DTYPE_CODE[dtype],
+                                         stream_ptr()), "cl3d_bn_relu_fwd")
     return y
 
 
 @_on_device
 def bn_relu_bwd(grad_y, x, stats, gamma, beta, training):
-    """-> (g_pm (B,M,Cp) point-major d/d(agg), dgamma (C,), dbeta (C,))"""
+    """grad_y in the features' dtype -> (g_pm (B,M,Cp) point-major d/d(agg), dgamma (C,), dbeta (C,)), all fp32"""
+    dt = require_features(grad_y, "grad_y")
     B, C, M = x.shape
     L = _lib.lib()
     dev = x.device
     partial = torch.empty(L.cl3d_agg_num_tiles(B, M), 2, C, dtype=F32, device=dev)
     dgb = torch.empty(2, C, dtype=F32, device=dev)
     g_pm = _empty_pm(B, M, padded_channels(C), dev)
-    check(L.cl3d_bn_relu_bwd(ptr(grad_y), ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, int(training),
-                             ptr(partial), ptr(dgb), ptr(g_pm), stream_ptr()), "cl3d_bn_relu_bwd")
+    check(L.cl3d_bn_relu_bwd_dt(ptr(grad_y), dt, ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, int(training),
+                                ptr(partial), ptr(dgb), ptr(g_pm), stream_ptr()), "cl3d_bn_relu_bwd")
     return g_pm, dgb[0], dgb[1]
 
 
@@ -285,12 +317,12 @@ def sgemm(a, sa_m, sa_k, b, sb_k, sb_n, M, N, K, out=None, ldc=None, splitk=1, a
 
 @_on_device
 def to_point_major_aug(x_cn, xyz, radius):
-    """(B,C,N) features + (B,N,3) xyz -> (B,N,Cpa) rows [f | xyz/r | 0], Cpa = padded(C+3)"""
-    require_cuda(x_cn, "features", F32)
+    """(B,C,N) f32 / f16 / bf16 features + (B,N,3) xyz -> (B,N,Cpa) fp32 rows [f | xyz/r | 0], Cpa = padded(C+3)"""
+    dt = require_features(x_cn, "features")
     B, C, N = x_cn.shape
     out = torch.empty(B, N, padded_channels(C + 3), dtype=F32, device=x_cn.device)
-    check(_lib.lib().cl3d_to_point_major_aug(ptr(x_cn), ptr(xyz), B, C, N, float(radius), ptr(out), stream_ptr()),
-          "cl3d_to_point_major_aug")
+    check(_lib.lib().cl3d_to_point_major_aug_dt(ptr(x_cn), dt, ptr(xyz), B, C, N, float(radius), ptr(out),
+                                                stream_ptr()), "cl3d_to_point_major_aug")
     return out
 
 
@@ -334,28 +366,30 @@ def pwmlp_fwd_stats(ab_pm, wp, sgn, query_xyz, support_xyz, idx, Cout, radius):
 
 
 @_on_device
-def pwmlp_fwd_out(ysel, stats, gamma, beta):
+def pwmlp_fwd_out(ysel, stats, gamma, beta, dtype=F32):
     B, Cout, M = ysel.shape
-    out = torch.empty_like(ysel)
-    check(_lib.lib().cl3d_pwmlp_fwd_out(ptr(ysel), ptr(stats), ptr(gamma), ptr(beta), B, M, Cout, ptr(out),
-                                        stream_ptr()), "cl3d_pwmlp_fwd_out")
+    out = torch.empty(B, Cout, M, dtype=dtype, device=ysel.device)
+    check(_lib.lib().cl3d_pwmlp_fwd_out_dt(ptr(ysel), ptr(stats), ptr(gamma), ptr(beta), B, M, Cout, ptr(out),
+                                           DTYPE_CODE[dtype], stream_ptr()), "cl3d_pwmlp_fwd_out")
     return out
 
 
 @_on_device
-def pwmlp_bwd(grad_out, out, ab_pm, wp, sgn, query_xyz, support_xyz, idx, csr_off, csr_ent, ysel, aq, sq, karg, stats, gamma,
-              radius, side_stream=None, training=True):
-    """-> (grad_ab_pm (B,N,2Cop), grad_wp (3,Cout), dgamma (Cout), dbeta (Cout)); side_stream: a torch stream the
-    library may fork onto (zero-fill + query pass run beside the gather pass), joined before it returns"""
+def pwmlp_bwd(grad_out, beta, ab_pm, wp, sgn, query_xyz, support_xyz, idx, csr_off, csr_ent, ysel, aq, sq, karg, stats,
+              gamma, radius, side_stream=None, training=True):
+    """grad_out in the features' dtype -> (grad_ab_pm (B,N,2Cop), grad_wp (3,Cout), dgamma (Cout), dbeta (Cout)), fp32;
+    the ReLU decision is recomputed from ysel, stats, gamma and beta.  side_stream: a torch stream the library may fork
+    onto (zero-fill + query pass run beside the gather pass), joined before it returns"""
+    dt = require_features(grad_out, "grad_out")
     B, N, C2 = ab_pm.shape
-    Cout, M, K = out.shape[1], out.shape[2], idx.shape[2]
+    Cout, M, K = ysel.shape[1], ysel.shape[2], idx.shape[2]
     L = _lib.lib()
-    dev = out.device
+    dev = ysel.device
     partial = _empty_pm(1, 1, L.cl3d_pwmlp_bwd_scratch_floats(B, N, M, Cout), dev)  # partial sums + sc*dz rows
     dgb = torch.empty(2, Cout, dtype=F32, device=dev)
     grad_ab = torch.empty(B, N, C2, dtype=F32, device=dev)
     grad_wp = torch.empty(3, Cout, dtype=F32, device=dev)
-    check(L.cl3d_pwmlp_bwd(ptr(grad_out), ptr(out), ptr(ab_pm), ptr(wp), ptr(sgn), ptr(query_xyz), ptr(support_xyz), ptr(idx),
+    check(L.cl3d_pwmlp_bwd_dt(ptr(grad_out), dt, ptr(beta), ptr(ab_pm), ptr(wp), ptr(sgn), ptr(query_xyz), ptr(support_xyz), ptr(idx),
                            ptr(csr_off), ptr(csr_ent), ptr(ysel), ptr(aq), ptr(sq), ptr(karg), ptr(stats), ptr(gamma),
                            B, N, M, K, Cout, float(radius), int(bool(training)), ptr(partial), ptr(dgb), ptr(grad_ab),
                            ptr(grad_wp),
@@ -387,27 +421,29 @@ def grid_subsample(points, mask, npoint, sampleDl):
 
 @_on_device
 def gather_max(features, idx):
-    """out[b,c,q] = max_k features[b,c,idx[b,q,k]] -> (out (B,C,M), arg (B,M,Cp) uint8)"""
-    require_cuda(features, "features", F32)
+    """out[b,c,q] = max_k features[b,c,idx[b,q,k]] -> (out (B,C,M) in the features' dtype, arg (B,M,Cp) uint8)"""
+    dt = require_features(features, "features")
     require_cuda(idx, "idx", I32)
     B, C, N = features.shape
     M, K = idx.shape[1], idx.shape[2]
     feat_pm = to_point_major(features)
-    out = torch.empty(B, C, M, dtype=F32, device=features.device)
+    out = torch.empty(B, C, M, dtype=features.dtype, device=features.device)
     arg = torch.empty(B, M, feat_pm.shape[2], dtype=torch.uint8, device=features.device)
-    check(_lib.lib().cl3d_gather_max_fwd(ptr(feat_pm), ptr(idx), B, N, M, K, C, ptr(out), ptr(arg), stream_ptr()),
-          "cl3d_gather_max_fwd")
+    check(_lib.lib().cl3d_gather_max_fwd_dt(ptr(feat_pm), ptr(idx), B, N, M, K, C, ptr(out), dt, ptr(arg),
+                                            stream_ptr()), "cl3d_gather_max_fwd")
     return out, arg
 
 
 @_on_device
 def gather_max_grad(grad_out, idx, arg, N):
+    """-> d/dfeatures (B,C,N) in grad_out's dtype (accumulated in fp32, rounded once)"""
+    dt = require_features(grad_out, "grad_out")
     B, C, M = grad_out.shape
     K = idx.shape[2]
     g_pm = torch.empty(B, N, padded_channels(C), dtype=F32, device=grad_out.device)
-    check(_lib.lib().cl3d_gather_max_bwd(ptr(grad_out), ptr(idx), ptr(arg), B, N, M, K, C, ptr(g_pm), stream_ptr()),
-          "cl3d_gather_max_bwd")
-    return to_channel_major(g_pm, C)
+    check(_lib.lib().cl3d_gather_max_bwd_dt(ptr(grad_out), dt, ptr(idx), ptr(arg), B, N, M, K, C, ptr(g_pm),
+                                            stream_ptr()), "cl3d_gather_max_bwd")
+    return to_channel_major(g_pm, C, grad_out.dtype)
 
 
 # ---- fused multi-shape part-segmentation head (multihead.cu) ------------------------------------------------------

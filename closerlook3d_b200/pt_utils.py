@@ -219,11 +219,13 @@ class GroupingOperation(Function):
     """pt_utils.py:16-61"""
 
     @staticmethod
+    @ops.no_autocast
     def forward(ctx, features, idx):
         ctx.for_backwards = (idx, features.size(2))
-        return ops.group_points(features.contiguous(), idx)
+        return ops.group_points(features.contiguous(), idx)   # in the features' dtype (fp32, fp16 or bf16)
 
     @staticmethod
+    @ops.no_autocast
     def backward(ctx, grad_out):
         idx, N = ctx.for_backwards
         return ops.group_points_grad(grad_out.contiguous(), idx, N), None
@@ -344,13 +346,15 @@ class _GatherMax(Function):
     """out[b,c,q] = max_k f[b,c,idx[b,q,k]]  (fused MaskedMaxPool body: pt_utils.py:195-201)"""
 
     @staticmethod
+    @ops.no_autocast
     def forward(ctx, features, idx):
-        out, arg = ops.gather_max(features, idx)
+        out, arg = ops.gather_max(features, idx)   # in the features' dtype; the winning slots decide the backward
         ctx.save_for_backward(idx, arg)
         ctx.N = features.shape[2]
         return out
 
     @staticmethod
+    @ops.no_autocast
     def backward(ctx, grad_out):
         idx, arg = ctx.saved_tensors
         return ops.gather_max_grad(grad_out.contiguous(), idx, arg, ctx.N), None

@@ -16,6 +16,7 @@ from . import ops, pt_utils
 
 class _FusedPointWiseMLP(Function):
     @staticmethod
+    @ops.no_autocast
     def forward(ctx, features, conv_weight, bn_weight, bn_bias, nl, query_xyz, support_xyz, radius, bn):
         B, C, N = features.shape
         M, K = nl.idx.shape[1], nl.idx.shape[2]
@@ -38,22 +39,25 @@ class _FusedPointWiseMLP(Function):
                 momentum = 1.0 / float(bn.num_batches_tracked)
         stats = ops.bn_finalize(partial, Cout, B * M * K, bn.eps, momentum, training, bn.running_mean,
                                 bn.running_var)
-        out = ops.pwmlp_fwd_out(ysel, stats, bn_weight, bn_bias)
+        out = ops.pwmlp_fwd_out(ysel, stats, bn_weight, bn_bias, dtype=features.dtype)
         ctx.nl, ctx.radius, ctx.training, ctx.dims = nl, radius, training, (B, C, N, M, K, Cout, Cop, Cpa)
-        ctx.save_for_backward(out, fa_pm, ab_pm, wp, sgn, wcat, ysel, aq, sq, karg, stats, bn_weight, query_xyz,
+        ctx.dtype = features.dtype
+        # the backward recomputes the ReLU decision from ysel and the BatchNorm constants, not from `out`
+        ctx.save_for_backward(fa_pm, ab_pm, wp, sgn, wcat, ysel, aq, sq, karg, stats, bn_weight, bn_bias, query_xyz,
                               support_xyz)
         return out
 
     @staticmethod
+    @ops.no_autocast
     def backward(ctx, grad_out):
-        (out, fa_pm, ab_pm, wp, sgn, wcat, ysel, aq, sq, karg, stats, bn_weight, query_xyz,
+        (fa_pm, ab_pm, wp, sgn, wcat, ysel, aq, sq, karg, stats, bn_weight, bn_bias, query_xyz,
          support_xyz) = ctx.saved_tensors
         B, C, N, M, K, Cout, Cop, Cpa = ctx.dims
         nl = ctx.nl
         # eval mode (frozen BatchNorm): no batch-statistics terms -> no dense pass, no transposed lists needed
         off, ent = nl.csr_all_slots() if ctx.training else (None, None)
-        side = pt_utils._side_stream(out.device, priority=-1) if pt_utils.overlap_enabled else None
-        grad_ab, grad_wp, dgamma, dbeta = ops.pwmlp_bwd(grad_out.contiguous(), out, ab_pm, wp, sgn, query_xyz, support_xyz, nl.idx,
+        side = pt_utils._side_stream(ysel.device, priority=-1) if pt_utils.overlap_enabled else None
+        grad_ab, grad_wp, dgamma, dbeta = ops.pwmlp_bwd(grad_out.contiguous(), bn_bias, ab_pm, wp, sgn, query_xyz, support_xyz, nl.idx,
                                                         off, ent, ysel, aq, sq, karg, stats, bn_weight, ctx.radius,
                                                         side_stream=side, training=ctx.training)
         P = B * N
@@ -69,7 +73,7 @@ class _FusedPointWiseMLP(Function):
             gW = ops.pwmlp_weight_grad(gwcat, grad_wp, sgn, C, Cout)
         # d/dfeat (point-major) = grad_AB (P x 2Cop) @ wcat[:, :Cp] (2Cop x Cp; columns >= C are unused)
         gf_pm = ops.sgemm(grad_ab, 2 * Cop, 1, wcat, Cpa, 1, P, Cp, 2 * Cop, ldc=Cp).view(B, N, Cp)
-        grad_feat = ops.to_channel_major(gf_pm, C)
+        grad_feat = ops.to_channel_major(gf_pm, C, ctx.dtype)
         cur.wait_stream(side)
         return grad_feat, gW, dgamma, dbeta, None, None, None, None, None
 

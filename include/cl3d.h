@@ -51,6 +51,14 @@ extern "C" {
 #define CL3D_FAM_ADAPTIVE_DP 2    /* AdaptiveWeight, weight_type='dp', num_mlps=1 (:188-197) */
 #define CL3D_FAM_PSEUDOGRID 3     /* PseudoGrid, linear / constant influence, sum (:368-419) */
 
+/* Element type of a channel-major feature tensor (the `_dt` entry points below).  Only the tensors that cross the
+ * channel-major <-> point-major boundary take it; inside, every buffer and every operation stays fp32.  A 16-bit
+ * input is widened exactly; an fp32 result is rounded once, to nearest even, where it is stored.  Unknown codes:
+ * CL3D_ERR_BAD_ARG.  Each fp32 entry point is its `_dt` twin with CL3D_DTYPE_F32. */
+#define CL3D_DTYPE_F32 0
+#define CL3D_DTYPE_F16 1
+#define CL3D_DTYPE_BF16 2
+
 typedef void* cl3d_stream_t; /* cudaStream_t */
 
 int cl3d_version(void);
@@ -133,6 +141,13 @@ int cl3d_group_points(const float* points /*(B,C,N)*/, const int* idx /*(B,M,K)*
  * summation order -- like the reference's group_points_grad_gpu.cu:48-69 -- is not deterministic (tolerance parity). */
 int cl3d_group_points_grad(const float* grad_out /*(B,C,M,K)*/, const int* idx, int B, int C, int N,
                            int M, int K, float* grad_points, cl3d_stream_t stream);
+/* points / out and grad_out / grad_points in `dtype`.  The 16-bit gradient is accumulated with fp32 atomics into
+ * `acc` (B*C*N floats of caller scratch; may be NULL for CL3D_DTYPE_F32, which accumulates in grad_points) and
+ * converted once. */
+int cl3d_group_points_dt(const void* points, int dtype, const int* idx, int B, int C, int N, int M, int K, void* out,
+                         cl3d_stream_t stream);
+int cl3d_group_points_grad_dt(const void* grad_out, int dtype, const int* idx, int B, int C, int N, int M, int K,
+                              void* grad_points, float* acc, cl3d_stream_t stream);
 
 /* Replaces _ext.masked_grid_subsampling (masked_grid_subsampling_gpu.cu:11-153).
  * sub_xyz (B,m,3) f32, sub_mask (B,m) i32. */
@@ -148,12 +163,20 @@ int cl3d_gather_max_fwd(const float* feat_pm, const int* idx, int B, int N, int 
                         unsigned char* arg, cl3d_stream_t stream);
 int cl3d_gather_max_bwd(const float* grad_out, const int* idx, const unsigned char* arg, int B, int N, int M,
                         int K, int C, float* grad_pm, cl3d_stream_t stream);
+/* out / grad_out in `dtype` (the maximum of exactly widened values is exact); feat_pm, grad_pm fp32 */
+int cl3d_gather_max_fwd_dt(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, void* out,
+                           int dtype, unsigned char* arg, cl3d_stream_t stream);
+int cl3d_gather_max_bwd_dt(const void* grad_out, int dtype, const int* idx, const unsigned char* arg, int B, int N,
+                           int M, int K, int C, float* grad_pm, cl3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Layout: channel-major (B,C,N) <-> point-major (B,N,Cp), Cp = cl3d_padded_channels(C), pad = 0.
  * ---------------------------------------------------------------------------------------------- */
 int cl3d_to_point_major(const float* in_cn, int B, int C, int N, float* out_nc, cl3d_stream_t stream);
 int cl3d_to_channel_major(const float* in_nc, int B, int C, int N, float* out_cn, cl3d_stream_t stream);
+/* the channel-major side in `dtype`; the point-major side fp32 */
+int cl3d_to_point_major_dt(const void* in_cn, int dtype, int B, int C, int N, float* out_nc, cl3d_stream_t stream);
+int cl3d_to_channel_major_dt(const float* in_nc, int B, int C, int N, void* out_cn, int dtype, cl3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused aggregation, families PosPool(xyz|sin_cos) / AdaptiveWeight(dp) / PseudoGrid.
@@ -196,6 +219,13 @@ int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const float* feat
                  int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
                  int influence, float* grad_feat, float* grad_params_partial,
                  const unsigned char* arg_pm, cl3d_stream_t stream);
+/* grad_feat written in `dtype` (by each backward kernel's own channel-major store); everything else as above */
+int cl3d_agg_bwd_dt(int family, int reduction, const float* g_pm, const float* feat_pm,
+                    const float* query_xyz, const float* support_xyz, const int* ncount,
+                    const int* csr_off, const int* csr_ent, const float* p0, const float* p1, int B, int N,
+                    int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
+                    int influence, void* grad_feat, int dtype, float* grad_params_partial,
+                    const unsigned char* arg_pm, cl3d_stream_t stream);
 /* out[p] = sum_t partial[t][p]  (fixed order -> deterministic given the partials) */
 int cl3d_reduce_partials(const float* partial, int ntiles, int P, float* out, cl3d_stream_t stream);
 
@@ -215,6 +245,12 @@ int cl3d_bn_relu_fwd(const float* x, const float* save_stats, const float* gamma
 int cl3d_bn_relu_bwd(const float* grad_y, const float* x, const float* save_stats, const float* gamma,
                      const float* beta, int B, int C, int M, int training, float* partial /*(ntiles,2,C)*/,
                      float* dgamma_dbeta /*(2,C)*/, float* g_pm /*(B,M,Cp)*/, cl3d_stream_t stream);
+/* y written / grad_y read in `dtype`; x, the statistics, partials, dgamma_dbeta and g_pm fp32 */
+int cl3d_bn_relu_fwd_dt(const float* x, const float* save_stats, const float* gamma, const float* beta,
+                        int B, int C, int M, void* y, int dtype, cl3d_stream_t stream);
+int cl3d_bn_relu_bwd_dt(const void* grad_y, int dtype, const float* x, const float* save_stats, const float* gamma,
+                        const float* beta, int B, int C, int M, int training, float* partial,
+                        float* dgamma_dbeta, float* g_pm, cl3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused PointWiseMLP (feature_type='dp_fi_df', num_mlps=1, reduction='max';
@@ -278,6 +314,19 @@ int cl3d_pwmlp_bwd(const float* grad_out, const float* out, const float* ab_pm, 
                    const unsigned char* karg, const float* save_stats, const float* gamma, int B, int N,
                    int M, int K, int Cout, float radius, int training, float* scratch, float* dgamma_dbeta,
                    float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream, cl3d_stream_t side_stream);
+/* in_cn / out / grad_out in `dtype`.  cl3d_pwmlp_bwd_dt takes beta instead of the stored output: the ReLU decision
+ * is recomputed from ysel, save_stats, gamma and beta with the forward's expression (bit-identical to the forward's
+ * fp32 decision; a 16-bit output may have rounded a small positive value to zero). */
+int cl3d_to_point_major_aug_dt(const void* in_cn, int dtype, const float* xyz, int B, int C, int N, float radius,
+                               float* out_nc, cl3d_stream_t stream);
+int cl3d_pwmlp_fwd_out_dt(const float* ysel, const float* save_stats, const float* gamma, const float* beta,
+                          int B, int M, int Cout, void* out, int dtype, cl3d_stream_t stream);
+int cl3d_pwmlp_bwd_dt(const void* grad_out, int dtype, const float* beta, const float* ab_pm, const float* wp,
+                      const float* sgn, const float* query_xyz, const float* support_xyz, const int* idx,
+                      const int* csr_off, const int* csr_ent, const float* ysel, const float* aq, const float* sq,
+                      const unsigned char* karg, const float* save_stats, const float* gamma, int B, int N,
+                      int M, int K, int Cout, float radius, int training, float* scratch, float* dgamma_dbeta,
+                      float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream, cl3d_stream_t side_stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused multi-shape part-segmentation head (multihead.cu).  Replaces the S per-shape heads of

@@ -5,6 +5,7 @@
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29533 \
         tools/train_synth.py --task scene_segmentation --la pospool_sincos --batch 8 --points 15000
     python tools/train_synth.py --task multi_part_segmentation --dataset shapenetpart --la pseudo_grid
+    python tools/train_synth.py --task scene_segmentation --la pseudo_grid --amp bf16
 
 The reference's training step (function/train_modelnet_dist.py:254-297, train_s3dis_dist.py): forward, loss,
 zero_grad, backward, SGD step, under DistributedDataParallel(broadcast_buffers=False) (:206); part segmentation as function/train_partnet_dist.py:274-282 (multi-shape
@@ -12,6 +13,8 @@ cross entropy on the list of per-shape logits, seeded shape and part labels) -- 
 networks (closerlook3d_b200/backbone.py: the reference's module tree on the fused neighbourhood operators).
 Synthetic data (no datasets in the container): points on noisy unit-sphere shells (surface-like density, so the
 shipped cfgs' radii see realistic neighbour counts), xyz (+1) as input features as the datasets provide them.
+--amp bf16 | fp16 runs forward and loss under torch.autocast (fp16 with a torch.amp.GradScaler); the fused operators
+take the 16-bit features autocast hands them and compute in fp32 inside.
 Prints one JSON line: whole-model points/s (device time, max over ranks) and a reference-format checkpoint round trip.
 """
 import argparse
@@ -57,6 +60,8 @@ def main():
     ap.add_argument("--ddp", action="store_true",
                     help="torch DistributedDataParallel (the reference's wrapper) instead of this package's flat "
                          "gradient buffer + one all-reduce per step (closerlook3d_b200/dist.py)")
+    ap.add_argument("--amp", default="off", choices=["off", "bf16", "fp16"],
+                    help="mixed precision: forward and loss under torch.autocast in this dtype (fp16 adds a GradScaler)")
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -98,29 +103,39 @@ def main():
     else:
         targets = [torch.randint(0, cfg.num_classes, (B, N), device=device) for _ in batches]
 
+    amp_dtype = {"off": None, "bf16": torch.bfloat16, "fp16": torch.float16}[args.amp]
+    scaler = torch.amp.GradScaler("cuda") if args.amp == "fp16" else None
+
     def step(i):
         xyz, mask, feats = batches[i % len(batches)]
-        pred = net(xyz, mask, feats)
-        if args.task == "classification":
-            loss = criterion(pred, targets[i % len(batches)])
-        elif part:
-            loss = criterion(pred, *targets[i % len(batches)])
-        else:
-            loss = criterion(pred, targets[i % len(batches)], mask.float())
+        with torch.autocast("cuda", dtype=amp_dtype or torch.float32, enabled=amp_dtype is not None):
+            pred = net(xyz, mask, feats)
+            if args.task == "classification":
+                loss = criterion(pred, targets[i % len(batches)])
+            elif part:
+                loss = criterion(pred, *targets[i % len(batches)])
+            else:
+                loss = criterion(pred, targets[i % len(batches)], mask.float())
+        scaled = scaler.scale(loss) if scaler is not None else loss
         if flat is not None:
             flat.zero()                 # the gradients are views of one buffer: one memset, one all-reduce
-            loss.backward()
+            scaled.backward()
             flat.allreduce()
         else:
             opt.zero_grad(set_to_none=True)
-            loss.backward()
-        opt.step()
+            scaled.backward()
+        if scaler is not None:
+            scaler.step(opt)
+            scaler.update()
+        else:
+            opt.step()
         return loss
 
     for i in range(args.warmup):
         step(i)
     pt_utils.cache_stats.update(hit=0, miss=0)
     torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats(device)
     if world > 1:
         dist.barrier()
     # one event per step boundary: mean AND median (a one-off stall -- allocator growth, a late NCCL channel set-up,
@@ -137,6 +152,7 @@ def main():
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms_mean, ms_median, ms_worst = (float(v) for v in ms.tolist())
+    peak_mb = torch.cuda.max_memory_allocated(device) / 2**20
     # checkpoint round trip in the reference's format (train_modelnet_dist.py:152-160: {'model': state_dict, ...})
     ok = None
     if rank == 0:
@@ -148,9 +164,11 @@ def main():
         fresh.load_state_dict(ck["model"], strict=True)
         ok = all(torch.equal(a.cpu(), b) for a, b in zip(model.state_dict().values(), fresh.state_dict().values()))
         print(json.dumps({"what": "whole-model training step (fwd + loss + bwd + SGD), synthetic clouds",
-                          "task": args.task, **({"dataset": args.dataset} if part else {}), "local_aggregation": args.la, "n_gpus": world, "clouds_per_gpu": B,
+                          "task": args.task, **({"dataset": args.dataset} if part else {}), "local_aggregation": args.la,
+                          "amp": args.amp, "n_gpus": world, "clouds_per_gpu": B,
                           "points_per_cloud": N, "steps": args.steps, "ms_per_step": ms_mean,
                           "ms_per_step_median": ms_median, "ms_slowest_step": ms_worst,
+                          "max_memory_allocated_MB": peak_mb,
                           "points_per_s": B * N * world / (ms_mean * 1e-3),
                           "points_per_s_median_step": B * N * world / (ms_median * 1e-3), "loss": float(loss.item()),
                           "neighbour_cache_per_step": {k: v / args.steps for k, v in pt_utils.cache_stats.items()},
