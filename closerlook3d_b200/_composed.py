@@ -1,7 +1,7 @@
 """Unfused GPU path for operator settings that no shipped cfg uses (output_conv / C_in != C_out, num_mlps > 1,
 gaussian influence, ...; the max reduction of PosPool / AdaptiveWeight is fused, csrc/agg_max.cu).  Same mathematics as the fused kernels and the reference
 (/root/reference/pytorch/models/local_aggregation_operators.py), built from this package's materialising
-kernels (MaskedQueryAndGroup -> cl3d_ball_query + cl3d_group_points) and torch library ops on the GPU.
+kernels (MaskedQueryAndGroup -> cl3d_ball_query_algo + cl3d_group_points) and torch library ops on the GPU.
 It exists so that every configuration the reference accepts runs here too; it is not the hot path.
 16-bit features are widened to fp32 and the result is rounded back to their dtype (autocast off throughout), like
 the fused operators.

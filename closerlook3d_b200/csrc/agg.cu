@@ -1004,12 +1004,12 @@ extern "C" int cl3d_agg_fwd(int family, int reduction, const float* feat_pm, con
   return dispatch_fwd(family, pick_ci(family, a.Cp), a, (cudaStream_t)stream_);
 }
 
-extern "C" int cl3d_agg_bwd_dt(int family, int reduction, const float* g_pm, const float* feat_pm,
-                               const float* query_xyz, const float* support_xyz, const int* ncount,
-                               const int* csr_off, const int* csr_ent, const float* p0, const float* p1, int B, int N,
-                               int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
-                               int influence, void* grad_feat, int dtype, float* grad_params_partial,
-                               const unsigned char* arg_pm, cl3d_stream_t stream_) {
+extern "C" int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const float* feat_pm,
+                            const float* query_xyz, const float* support_xyz, const int* ncount,
+                            const int* csr_off, const int* csr_ent, const float* p0, const float* p1, int B, int N,
+                            int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
+                            int influence, void* grad_feat, int dtype, float* grad_params_partial,
+                            const unsigned char* arg_pm, cl3d_stream_t stream_) {
   int rc = check_common(family, reduction, B, N, M, K, C, shared, nkp);
   if (rc) return rc;
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_agg_bwd");
@@ -1041,15 +1041,4 @@ extern "C" int cl3d_agg_bwd_dt(int family, int reduction, const float* g_pm, con
   if (family == CL3D_FAM_PSEUDOGRID && pg2_supported(a))
     return pg2_launch_bwd(a, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
   return dispatch_bwd(family, pick_ci(family, a.Cp), a, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
-}
-
-extern "C" int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const float* feat_pm,
-                            const float* query_xyz, const float* support_xyz, const int* ncount,
-                            const int* csr_off, const int* csr_ent, const float* p0, const float* p1, int B, int N,
-                            int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
-                            int influence, float* grad_feat, float* grad_params_partial,
-                            const unsigned char* arg_pm, cl3d_stream_t stream_) {
-  return cl3d_agg_bwd_dt(family, reduction, g_pm, feat_pm, query_xyz, support_xyz, ncount, csr_off, csr_ent, p0, p1,
-                         B, N, M, K, C, radius, normalize, shared, nkp, extent, influence, grad_feat, CL3D_DTYPE_F32,
-                         grad_params_partial, arg_pm, stream_);
 }

@@ -260,8 +260,8 @@ extern "C" int cl3d_bn_finalize(const float* bn_partial, int ntiles, int C, long
   return check_launch("bn_finalize_kernel");
 }
 
-extern "C" int cl3d_bn_relu_fwd_dt(const float* x, const float* save_stats, const float* gamma, const float* beta,
-                                   int B, int C, int M, void* y, int dtype, cl3d_stream_t stream_) {
+extern "C" int cl3d_bn_relu_fwd(const float* x, const float* save_stats, const float* gamma, const float* beta,
+                                int B, int C, int M, void* y, int dtype, cl3d_stream_t stream_) {
   CL3D_REQUIRE(x && save_stats && gamma && beta && y && B >= 0 && C >= 1 && M >= 1, "cl3d_bn_relu_fwd: bad arguments");
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_bn_relu_fwd");
   if (B == 0) return CL3D_OK;
@@ -276,14 +276,9 @@ extern "C" int cl3d_bn_relu_fwd_dt(const float* x, const float* save_stats, cons
   });
 }
 
-extern "C" int cl3d_bn_relu_fwd(const float* x, const float* save_stats, const float* gamma, const float* beta, int B,
-                                int C, int M, float* y, cl3d_stream_t stream_) {
-  return cl3d_bn_relu_fwd_dt(x, save_stats, gamma, beta, B, C, M, y, CL3D_DTYPE_F32, stream_);
-}
-
-extern "C" int cl3d_bn_relu_bwd_dt(const void* grad_y, int dtype, const float* x, const float* save_stats,
-                                   const float* gamma, const float* beta, int B, int C, int M, int training,
-                                   float* partial, float* dgamma_dbeta, float* g_pm, cl3d_stream_t stream_) {
+extern "C" int cl3d_bn_relu_bwd(const void* grad_y, int dtype, const float* x, const float* save_stats,
+                                const float* gamma, const float* beta, int B, int C, int M, int training,
+                                float* partial, float* dgamma_dbeta, float* g_pm, cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(grad_y && x && save_stats && gamma && beta && partial && dgamma_dbeta && g_pm,
                "cl3d_bn_relu_bwd: null pointer");
@@ -301,11 +296,4 @@ extern "C" int cl3d_bn_relu_bwd_dt(const void* grad_y, int dtype, const float* x
                                                             1.0f / (float)((long long)B * M), training, g_pm); CL3D_LAUNCHED(1);
     return check_launch("bn_relu_bwd kernels");
   });
-}
-
-extern "C" int cl3d_bn_relu_bwd(const float* grad_y, const float* x, const float* save_stats, const float* gamma,
-                                const float* beta, int B, int C, int M, int training, float* partial,
-                                float* dgamma_dbeta, float* g_pm, cl3d_stream_t stream_) {
-  return cl3d_bn_relu_bwd_dt(grad_y, CL3D_DTYPE_F32, x, save_stats, gamma, beta, B, C, M, training, partial,
-                             dgamma_dbeta, g_pm, stream_);
 }

@@ -173,14 +173,14 @@ __global__ void __launch_bounds__(1024) reduce_partials_kernel(const float* __re
 
 using namespace cl3d;
 
-extern "C" int cl3d_version(void) { return 100; }
+extern "C" int cl3d_version(void) { return 101; }
 extern "C" const char* cl3d_last_error(void) { return g_err; }
 extern "C" int cl3d_padded_channels(int C) { return padded_channels(C); }
 extern "C" int cl3d_sm_count(void) { return sm_count(); }
 extern "C" long long cl3d_launch_count(void) { return __atomic_load_n(&g_launches, __ATOMIC_RELAXED); }
 
-extern "C" int cl3d_to_point_major_dt(const void* in_cn, int dtype, int B, int C, int N, float* out_nc,
-                                      cl3d_stream_t stream_) {
+extern "C" int cl3d_to_point_major(const void* in_cn, int dtype, int B, int C, int N, float* out_nc,
+                                   cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && in_cn && out_nc, "cl3d_to_point_major: bad arguments");
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_to_point_major");
@@ -194,12 +194,8 @@ extern "C" int cl3d_to_point_major_dt(const void* in_cn, int dtype, int B, int C
   });
 }
 
-extern "C" int cl3d_to_point_major(const float* in_cn, int B, int C, int N, float* out_nc, cl3d_stream_t stream_) {
-  return cl3d_to_point_major_dt(in_cn, CL3D_DTYPE_F32, B, C, N, out_nc, stream_);
-}
-
-extern "C" int cl3d_to_channel_major_dt(const float* in_nc, int B, int C, int N, void* out_cn, int dtype,
-                                        cl3d_stream_t stream_) {
+extern "C" int cl3d_to_channel_major(const float* in_nc, int B, int C, int N, void* out_cn, int dtype,
+                                     cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && in_nc && out_cn, "cl3d_to_channel_major: bad arguments");
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_to_channel_major");
@@ -213,12 +209,8 @@ extern "C" int cl3d_to_channel_major_dt(const float* in_nc, int B, int C, int N,
   });
 }
 
-extern "C" int cl3d_to_channel_major(const float* in_nc, int B, int C, int N, float* out_cn, cl3d_stream_t stream_) {
-  return cl3d_to_channel_major_dt(in_nc, B, C, N, out_cn, CL3D_DTYPE_F32, stream_);
-}
-
-extern "C" int cl3d_group_points_dt(const void* points, int dtype, const int* idx, int B, int C, int N, int M, int K,
-                                    void* out, cl3d_stream_t stream_) {
+extern "C" int cl3d_group_points(const void* points, int dtype, const int* idx, int B, int C, int N, int M, int K,
+                                 void* out, cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && M >= 0 && K >= 1 && points && idx && out, "cl3d_group_points: bad arguments");
   CL3D_REQUIRE(C <= 65535 && B <= 65535, "cl3d_group_points: C or B too large");
@@ -234,13 +226,8 @@ extern "C" int cl3d_group_points_dt(const void* points, int dtype, const int* id
   });
 }
 
-extern "C" int cl3d_group_points(const float* points, const int* idx, int B, int C, int N, int M, int K, float* out,
-                                 cl3d_stream_t stream_) {
-  return cl3d_group_points_dt(points, CL3D_DTYPE_F32, idx, B, C, N, M, K, out, stream_);
-}
-
-extern "C" int cl3d_group_points_grad_dt(const void* grad_out, int dtype, const int* idx, int B, int C, int N, int M,
-                                         int K, void* grad_points, float* acc, cl3d_stream_t stream_) {
+extern "C" int cl3d_group_points_grad(const void* grad_out, int dtype, const int* idx, int B, int C, int N, int M,
+                                      int K, void* grad_points, float* acc, cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && M >= 0 && K >= 1 && grad_out && idx && grad_points,
                "cl3d_group_points_grad: bad arguments");
@@ -267,11 +254,6 @@ extern "C" int cl3d_group_points_grad_dt(const void* grad_out, int dtype, const 
     }
     return check_launch("group_points_grad_kernel");
   });
-}
-
-extern "C" int cl3d_group_points_grad(const float* grad_out, const int* idx, int B, int C, int N, int M, int K,
-                                      float* grad_points, cl3d_stream_t stream_) {
-  return cl3d_group_points_grad_dt(grad_out, CL3D_DTYPE_F32, idx, B, C, N, M, K, grad_points, nullptr, stream_);
 }
 
 extern "C" int cl3d_reduce_partials(const float* partial, int ntiles, int P, float* out, cl3d_stream_t stream_) {

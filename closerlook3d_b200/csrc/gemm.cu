@@ -329,10 +329,3 @@ extern "C" int cl3d_sgemm_algo(const float* a, long long sa_m, long long sa_k, c
   }
   return sgemm_ffma(a, sa_m, sa_k, b, sb_k, sb_n, M, N, K, c, ldc, splitk, partial, stream);
 }
-
-extern "C" int cl3d_sgemm(const float* a, long long sa_m, long long sa_k, const float* b, long long sb_k,
-                          long long sb_n, int M, int N, int K, float* c, long long ldc, int splitk, void* workspace,
-                          size_t workspace_bytes, cl3d_stream_t stream_) {
-  return cl3d_sgemm_algo(a, sa_m, sa_k, b, sb_k, sb_n, M, N, K, c, ldc, splitk, workspace, workspace_bytes,
-                         CL3D_GEMM_AUTO, stream_);
-}

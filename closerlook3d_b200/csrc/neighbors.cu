@@ -1,9 +1,9 @@
 // neighbors.cu -- neighbour search for the local-aggregation engine (sm_90a).
 //
-//   cl3d_ball_query    bit-exact replacement of the reference's masked_ordered_ball_query
-//                      (/root/reference/pytorch/ops/pt_custom_ops/_ext_src/src/masked_ordered_ball_query_gpu.cu:11-96)
-//   cl3d_nearest_query bit-exact replacement of masked_nearest_query (masked_nearest_query_gpu.cu:8-62)
-//   cl3d_build_csr     transposed neighbour lists for the gather-form backward kernels
+//   cl3d_ball_query_algo  bit-exact replacement of the reference's masked_ordered_ball_query
+//                         (/root/reference/pytorch/ops/pt_custom_ops/_ext_src/src/masked_ordered_ball_query_gpu.cu:11-96)
+//   cl3d_nearest_query    bit-exact replacement of masked_nearest_query (masked_nearest_query_gpu.cu:8-62)
+//   cl3d_build_csr        transposed neighbour lists for the gather-form backward kernels
 //
 // The reference scans ALL support points per query on B thread blocks.  Here the support cloud is binned
 // into a uniform grid (cell edge >= radius, counting sort, points stored as float4 {x,y,z,index} in cell
@@ -987,14 +987,6 @@ extern "C" size_t cl3d_ball_query_workspace_bytes(int B, int N, int M, int K) {
   s += align_up(sizeof(int2) * (size_t)B * N, 256);         // cell id + rank
   s += align_up(sizeof(float4) * (size_t)B * N, 256);       // cell-sorted points
   return s;
-}
-
-extern "C" int cl3d_ball_query(const float* query_xyz, const float* support_xyz, const int* query_mask,
-                               const int* support_mask, int B, int N, int M, float radius, int K, int* idx,
-                               int* idx_mask, int* ncount, void* workspace, size_t workspace_bytes,
-                               cl3d_stream_t stream_) {
-  return cl3d_ball_query_algo(query_xyz, support_xyz, query_mask, support_mask, B, N, M, radius, K, idx, idx_mask,
-                              ncount, workspace, workspace_bytes, CL3D_BQ_AUTO, stream_);
 }
 
 static int ball_query_impl(const float* query_xyz, const float* support_xyz, const int* query_mask,

@@ -128,8 +128,8 @@ static int launch_pool_fwd(const float* feat_pm, const int* idx, int B, int N, i
 
 using namespace cl3d;
 
-extern "C" int cl3d_gather_max_fwd_dt(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C,
-                                      void* out, int dtype, unsigned char* arg, cl3d_stream_t stream_) {
+extern "C" int cl3d_gather_max_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C,
+                                   void* out, int dtype, unsigned char* arg, cl3d_stream_t stream_) {
   CL3D_REQUIRE(feat_pm && idx && out && arg && B >= 0 && N >= 1 && M >= 1 && K >= 1 && K <= 255 && C >= 1,
                "cl3d_gather_max_fwd: bad arguments (K <= 255)");
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_gather_max_fwd");
@@ -150,13 +150,8 @@ extern "C" int cl3d_gather_max_fwd_dt(const float* feat_pm, const int* idx, int 
   });
 }
 
-extern "C" int cl3d_gather_max_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, float* out,
-                                   unsigned char* arg, cl3d_stream_t stream_) {
-  return cl3d_gather_max_fwd_dt(feat_pm, idx, B, N, M, K, C, out, CL3D_DTYPE_F32, arg, stream_);
-}
-
-extern "C" int cl3d_gather_max_bwd_dt(const void* grad_out, int dtype, const int* idx, const unsigned char* arg, int B,
-                                      int N, int M, int K, int C, float* grad_pm, cl3d_stream_t stream_) {
+extern "C" int cl3d_gather_max_bwd(const void* grad_out, int dtype, const int* idx, const unsigned char* arg, int B,
+                                   int N, int M, int K, int C, float* grad_pm, cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(grad_out && idx && arg && grad_pm && B >= 0 && N >= 1 && M >= 1 && K >= 1 && C >= 1,
                "cl3d_gather_max_bwd: bad arguments");
@@ -174,9 +169,4 @@ extern "C" int cl3d_gather_max_bwd_dt(const void* grad_out, int dtype, const int
     CL3D_LAUNCHED(1);
     return check_launch("gather_max_bwd_kernel");
   });
-}
-
-extern "C" int cl3d_gather_max_bwd(const float* grad_out, const int* idx, const unsigned char* arg, int B, int N,
-                                   int M, int K, int C, float* grad_pm, cl3d_stream_t stream_) {
-  return cl3d_gather_max_bwd_dt(grad_out, CL3D_DTYPE_F32, idx, arg, B, N, M, K, C, grad_pm, stream_);
 }

@@ -47,8 +47,8 @@ struct PwArgs {
   unsigned char* karg;       // (B,M,Cop) first arg-max slot
   float* partial;            // fwd: (ntiles,2,Cout) ; bwd sparse: (ntiles,3,Cout) dWp partials
   // backward only
-  const float* grad_out;     // unused (kept for the layout of this block): pwmlp_bwd_stats_kernel, the only reader
-  const float* out;          // of grad_out / out, takes them as kernel arguments
+  const float* grad_out;     // unused, kept for the layout of this block: pwmlp_bwd_stats_kernel takes grad_out as
+  const float* out;          // a kernel argument, and nothing reads out
   const float* stats;        // (2,Cout) mean, invstd
   const float* gamma;        // (Cout)
   const float* dgb;          // (2,Cout): sum dz*yhat, sum dz
@@ -229,7 +229,7 @@ __global__ void __launch_bounds__(256) pwmlp_out_kernel(const float* __restrict_
   const float* src = ysel + (size_t)row * M;
   T* dst = out + (size_t)row * M;
   for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < M; i += gridDim.y * blockDim.x) {
-    const float v = __fmaf_rn(__fsub_rn(src[i], mean), sc, sh);  // pwmlp_bwd_stats_kernel<., true> recomputes this
+    const float v = __fmaf_rn(__fsub_rn(src[i], mean), sc, sh);  // pwmlp_bwd_stats_kernel recomputes this
     store_f32(dst + i, v > 0.f ? v : 0.f);
   }
 }
@@ -237,12 +237,11 @@ __global__ void __launch_bounds__(256) pwmlp_out_kernel(const float* __restrict_
 // =================================================================================================
 // backward
 // =================================================================================================
-// FROM_YSEL = false: the ReLU passed where the stored fp32 output is positive.  true: the decision is recomputed from
-// ysel and the BatchNorm constants with pwmlp_out_kernel's expression (a 16-bit output can round a small positive
-// value to zero, so it cannot decide).  Both give the forward's fp32 decision bit for bit.
-template <typename TG, bool FROM_YSEL>
+// The ReLU decision is recomputed from ysel and the BatchNorm constants with pwmlp_out_kernel's expression, which gives
+// the forward's fp32 decision bit for bit (a 16-bit output can round a small positive value to zero, so it cannot
+// decide).
+template <typename TG>
 __global__ void __launch_bounds__(256) pwmlp_bwd_stats_kernel(const TG* __restrict__ grad_out,
-                                                              const float* __restrict__ out,
                                                               const float* __restrict__ ysel,
                                                               const float* __restrict__ stats,
                                                               const float* __restrict__ gamma, int C, int Cop, int M,
@@ -259,9 +258,7 @@ __global__ void __launch_bounds__(256) pwmlp_bwd_stats_kernel(const TG* __restri
     float dz = 0.f, dzy = 0.f, sc = 0.f;
     if (c < C && q < M) {
       const size_t o = ((size_t)b * C + c) * M + q;
-      bool pass;
-      if constexpr (FROM_YSEL) pass = __fmaf_rn(__fsub_rn(ysel[o], stats[c]), stats[C + c] * gamma[c], beta[c]) > 0.f;
-      else pass = out[o] > 0.f;
+      const bool pass = __fmaf_rn(__fsub_rn(ysel[o], stats[c]), stats[C + c] * gamma[c], beta[c]) > 0.f;
       dz = pass ? load_f32(grad_out + o) : 0.f;
       dzy = dz * ((ysel[o] - stats[c]) * stats[C + c]);
       sc = stats[C + c] * gamma[c];
@@ -544,8 +541,8 @@ static int pw_query_grid(int B, int M, int Cop) {
 
 using namespace cl3d;
 
-extern "C" int cl3d_to_point_major_aug_dt(const void* in_cn, int dtype, const float* xyz, int B, int C, int N,
-                                          float radius, float* out_nc, cl3d_stream_t stream_) {
+extern "C" int cl3d_to_point_major_aug(const void* in_cn, int dtype, const float* xyz, int B, int C, int N,
+                                       float radius, float* out_nc, cl3d_stream_t stream_) {
   CL3D_REQUIRE(in_cn && xyz && out_nc && B >= 0 && C >= 1 && N >= 1, "cl3d_to_point_major_aug: bad arguments");
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_to_point_major_aug");
   if (B == 0) return CL3D_OK;
@@ -558,11 +555,6 @@ extern "C" int cl3d_to_point_major_aug_dt(const void* in_cn, int dtype, const fl
     CL3D_LAUNCHED(1);
     return check_launch("to_point_major_aug_kernel");
   });
-}
-
-extern "C" int cl3d_to_point_major_aug(const float* in_cn, const float* xyz, int B, int C, int N, float radius,
-                                       float* out_nc, cl3d_stream_t stream_) {
-  return cl3d_to_point_major_aug_dt(in_cn, CL3D_DTYPE_F32, xyz, B, C, N, radius, out_nc, stream_);
 }
 
 extern "C" int cl3d_pwmlp_prep_weights(const float* conv_weight, const float* gamma, int C, int Cout, float* wcat,
@@ -607,8 +599,8 @@ extern "C" int cl3d_pwmlp_fwd_stats(const float* ab_pm, const float* wp, const f
   }
 }
 
-extern "C" int cl3d_pwmlp_fwd_out_dt(const float* ysel, const float* save_stats, const float* gamma, const float* beta,
-                                     int B, int M, int Cout, void* out, int dtype, cl3d_stream_t stream_) {
+extern "C" int cl3d_pwmlp_fwd_out(const float* ysel, const float* save_stats, const float* gamma, const float* beta,
+                                  int B, int M, int Cout, void* out, int dtype, cl3d_stream_t stream_) {
   CL3D_REQUIRE(ysel && save_stats && gamma && beta && out && B >= 0 && M >= 1 && Cout >= 1,
                "cl3d_pwmlp_fwd_out: bad arguments");
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_pwmlp_fwd_out");
@@ -622,11 +614,6 @@ extern "C" int cl3d_pwmlp_fwd_out_dt(const float* ysel, const float* save_stats,
     CL3D_LAUNCHED(1);
     return check_launch("pwmlp_out_kernel");
   });
-}
-
-extern "C" int cl3d_pwmlp_fwd_out(const float* ysel, const float* save_stats, const float* gamma, const float* beta,
-                                  int B, int M, int Cout, float* out, cl3d_stream_t stream_) {
-  return cl3d_pwmlp_fwd_out_dt(ysel, save_stats, gamma, beta, B, M, Cout, out, CL3D_DTYPE_F32, stream_);
 }
 
 extern "C" size_t cl3d_pwmlp_bwd_scratch_floats(int B, int N, int M, int Cout) {
@@ -662,15 +649,13 @@ static PwEvents* pw_events() {
   return &ring[dev][next[dev]++ % kRing];
 }
 
-// the ReLU of the statistics pass is decided by the stored fp32 output `out` (cl3d_pwmlp_bwd) or, when out is NULL,
-// recomputed from ysel and beta (cl3d_pwmlp_bwd_dt)
-static int pwmlp_bwd(const void* grad_out, int dtype, const float* out, const float* beta, const float* ab_pm,
-                     const float* wp, const float* sgn, const float* query_xyz, const float* support_xyz, const int* idx,
-                     const int* csr_off, const int* csr_ent, const float* ysel, const float* aq, const float* sq,
-                     const unsigned char* karg, const float* save_stats, const float* gamma, int B, int N,
-                     int M, int K, int Cout, float radius, int training, float* scratch,
-                     float* dgamma_dbeta, float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream_,
-                     cl3d_stream_t side_stream_) {
+extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta, const float* ab_pm,
+                              const float* wp, const float* sgn, const float* query_xyz, const float* support_xyz,
+                              const int* idx, const int* csr_off, const int* csr_ent, const float* ysel,
+                              const float* aq, const float* sq, const unsigned char* karg, const float* save_stats,
+                              const float* gamma, int B, int N, int M, int K, int Cout, float radius, int training,
+                              float* scratch, float* dgamma_dbeta, float* grad_ab_pm, float* grad_wp,
+                              cl3d_stream_t stream_, cl3d_stream_t side_stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   // With a side stream the zero-fill of grad_ab and the latency-bound query pass run beside the statistics and
   // the support-major gather (fork/join with events: capturable into a CUDA graph); without one, in order.
@@ -679,7 +664,7 @@ static int pwmlp_bwd(const void* grad_out, int dtype, const float* out, const fl
   PwEvents* ev = forked ? pw_events() : nullptr;
   if (forked && !ev) return CL3D_ERR_LAUNCH;
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_pwmlp_bwd");
-  CL3D_REQUIRE(grad_out && (out || beta) && ab_pm && wp && sgn && query_xyz && support_xyz && idx && ysel && aq && sq &&
+  CL3D_REQUIRE(grad_out && beta && ab_pm && wp && sgn && query_xyz && support_xyz && idx && ysel && aq && sq &&
                    karg && save_stats && gamma && scratch && dgamma_dbeta && grad_ab_pm && grad_wp,
                "cl3d_pwmlp_bwd: null pointer");
   CL3D_REQUIRE(!training || (csr_off && csr_ent), "cl3d_pwmlp_bwd: training mode needs the all-slots CSR lists");
@@ -704,17 +689,10 @@ static int pwmlp_bwd(const void* grad_out, int dtype, const float* out, const fl
   with_dtype(dtype, [&](auto t) {
     using TG = typename decltype(t)::type;
     const TG* g = static_cast<const TG*>(grad_out);
-    if (out) {
-      static std::atomic<unsigned long long> seen_stats{0};
-      allow_big_smem(pwmlp_bwd_stats_kernel<TG, false>, seen_stats);
-      pwmlp_bwd_stats_kernel<TG, false><<<ntiles, 256, smem_s, stream>>>(g, out, ysel, save_stats, gamma, Cout, Cop, M,
-                                                                         partial, dzs_pm, beta);
-    } else {
-      static std::atomic<unsigned long long> seen_stats{0};
-      allow_big_smem(pwmlp_bwd_stats_kernel<TG, true>, seen_stats);
-      pwmlp_bwd_stats_kernel<TG, true><<<ntiles, 256, smem_s, stream>>>(g, out, ysel, save_stats, gamma, Cout, Cop, M,
-                                                                        partial, dzs_pm, beta);
-    }
+    static std::atomic<unsigned long long> seen_stats{0};
+    allow_big_smem(pwmlp_bwd_stats_kernel<TG>, seen_stats);
+    pwmlp_bwd_stats_kernel<TG><<<ntiles, 256, smem_s, stream>>>(g, ysel, save_stats, gamma, Cout, Cop, M, partial, dzs_pm,
+                                                                beta);
     return CL3D_OK;
   });
   CL3D_LAUNCHED(1);
@@ -761,28 +739,4 @@ static int pwmlp_bwd(const void* grad_out, int dtype, const float* out, const fl
     cudaStreamWaitEvent(stream, ev->joined, 0);
   }
   return rc;
-}
-
-extern "C" int cl3d_pwmlp_bwd(const float* grad_out, const float* out, const float* ab_pm, const float* wp,
-                              const float* sgn, const float* query_xyz, const float* support_xyz, const int* idx,
-                              const int* csr_off, const int* csr_ent, const float* ysel, const float* aq, const float* sq,
-                              const unsigned char* karg, const float* save_stats, const float* gamma, int B, int N,
-                              int M, int K, int Cout, float radius, int training, float* scratch,
-                              float* dgamma_dbeta, float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream_,
-                              cl3d_stream_t side_stream_) {
-  return pwmlp_bwd(grad_out, CL3D_DTYPE_F32, out, nullptr, ab_pm, wp, sgn, query_xyz, support_xyz, idx, csr_off, csr_ent,
-                   ysel, aq, sq, karg, save_stats, gamma, B, N, M, K, Cout, radius, training, scratch, dgamma_dbeta,
-                   grad_ab_pm, grad_wp, stream_, side_stream_);
-}
-
-extern "C" int cl3d_pwmlp_bwd_dt(const void* grad_out, int dtype, const float* beta, const float* ab_pm,
-                                 const float* wp, const float* sgn, const float* query_xyz, const float* support_xyz,
-                                 const int* idx, const int* csr_off, const int* csr_ent, const float* ysel,
-                                 const float* aq, const float* sq, const unsigned char* karg, const float* save_stats,
-                                 const float* gamma, int B, int N, int M, int K, int Cout, float radius, int training,
-                                 float* scratch, float* dgamma_dbeta, float* grad_ab_pm, float* grad_wp,
-                                 cl3d_stream_t stream_, cl3d_stream_t side_stream_) {
-  return pwmlp_bwd(grad_out, dtype, nullptr, beta, ab_pm, wp, sgn, query_xyz, support_xyz, idx, csr_off, csr_ent, ysel,
-                   aq, sq, karg, save_stats, gamma, B, N, M, K, Cout, radius, training, scratch, dgamma_dbeta,
-                   grad_ab_pm, grad_wp, stream_, side_stream_);
 }

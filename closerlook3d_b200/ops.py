@@ -159,7 +159,7 @@ def to_point_major(x_cn):
     dt = require_features(x_cn, "features")
     B, C, N = x_cn.shape
     out = _empty_pm(B, N, padded_channels(C), x_cn.device)
-    check(_lib.lib().cl3d_to_point_major_dt(ptr(x_cn), dt, B, C, N, ptr(out), stream_ptr()), "cl3d_to_point_major")
+    check(_lib.lib().cl3d_to_point_major(ptr(x_cn), dt, B, C, N, ptr(out), stream_ptr()), "cl3d_to_point_major")
     return out
 
 
@@ -169,7 +169,7 @@ def to_channel_major(x_nc, C, dtype=F32):
     B, N, Cp = x_nc.shape
     assert Cp == padded_channels(C)
     out = torch.empty(B, C, N, dtype=dtype, device=x_nc.device)
-    check(_lib.lib().cl3d_to_channel_major_dt(ptr(x_nc), B, C, N, ptr(out), DTYPE_CODE[dtype], stream_ptr()),
+    check(_lib.lib().cl3d_to_channel_major(ptr(x_nc), B, C, N, ptr(out), DTYPE_CODE[dtype], stream_ptr()),
           "cl3d_to_channel_major")
     return out
 
@@ -181,7 +181,7 @@ def group_points(points, idx):
     B, C, N = points.shape
     _, M, K = idx.shape
     out = torch.empty(B, C, M, K, dtype=points.dtype, device=points.device)
-    check(_lib.lib().cl3d_group_points_dt(ptr(points), dt, ptr(idx), B, C, N, M, K, ptr(out), stream_ptr()),
+    check(_lib.lib().cl3d_group_points(ptr(points), dt, ptr(idx), B, C, N, M, K, ptr(out), stream_ptr()),
           "cl3d_group_points")
     return out
 
@@ -194,8 +194,8 @@ def group_points_grad(grad_out, idx, n):
     B, C, M, K = grad_out.shape
     out = torch.empty(B, C, int(n), dtype=grad_out.dtype, device=grad_out.device)
     acc = torch.empty(B, C, int(n), dtype=F32, device=grad_out.device) if dt else None
-    check(_lib.lib().cl3d_group_points_grad_dt(ptr(grad_out), dt, ptr(idx), B, C, int(n), M, K, ptr(out), ptr(acc),
-                                               stream_ptr()), "cl3d_group_points_grad")
+    check(_lib.lib().cl3d_group_points_grad(ptr(grad_out), dt, ptr(idx), B, C, int(n), M, K, ptr(out), ptr(acc),
+                                            stream_ptr()), "cl3d_group_points_grad")
     return out
 
 
@@ -248,10 +248,10 @@ def agg_bwd(family, reduction, g_pm, feat_pm, query_xyz, support_xyz, ncount, cs
     partial = None
     if P > 0:
         partial = torch.empty(L.cl3d_agg_bwd_num_blocks(B, N), P, dtype=F32, device=dev)
-    check(L.cl3d_agg_bwd_dt(family, reduction, ptr(g_pm), ptr(feat_pm), ptr(query_xyz), ptr(support_xyz), ptr(ncount),
-                            ptr(csr_off), ptr(csr_ent), ptr(p0), ptr(p1), B, N, M, K, C, float(radius), int(normalize),
-                            int(shared), int(nkp), float(extent), int(influence), ptr(grad_feat), DTYPE_CODE[dtype],
-                            ptr(partial), ptr(arg), stream_ptr()), "cl3d_agg_bwd")
+    check(L.cl3d_agg_bwd(family, reduction, ptr(g_pm), ptr(feat_pm), ptr(query_xyz), ptr(support_xyz), ptr(ncount),
+                         ptr(csr_off), ptr(csr_ent), ptr(p0), ptr(p1), B, N, M, K, C, float(radius), int(normalize),
+                         int(shared), int(nkp), float(extent), int(influence), ptr(grad_feat), DTYPE_CODE[dtype],
+                         ptr(partial), ptr(arg), stream_ptr()), "cl3d_agg_bwd")
     pg = reduce_partials(partial).view(P // C, C) if P > 0 else None
     return grad_feat, pg
 
@@ -273,8 +273,8 @@ def bn_relu_fwd(x, stats, gamma, beta, dtype=F32):
     """x (B,C,M) fp32 -> y in `dtype`"""
     B, C, M = x.shape
     y = torch.empty(B, C, M, dtype=dtype, device=x.device)
-    check(_lib.lib().cl3d_bn_relu_fwd_dt(ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, ptr(y), DTYPE_CODE[dtype],
-                                         stream_ptr()), "cl3d_bn_relu_fwd")
+    check(_lib.lib().cl3d_bn_relu_fwd(ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, ptr(y), DTYPE_CODE[dtype],
+                                      stream_ptr()), "cl3d_bn_relu_fwd")
     return y
 
 
@@ -288,8 +288,8 @@ def bn_relu_bwd(grad_y, x, stats, gamma, beta, training):
     partial = torch.empty(L.cl3d_agg_num_tiles(B, M), 2, C, dtype=F32, device=dev)
     dgb = torch.empty(2, C, dtype=F32, device=dev)
     g_pm = _empty_pm(B, M, padded_channels(C), dev)
-    check(L.cl3d_bn_relu_bwd_dt(ptr(grad_y), dt, ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, int(training),
-                                ptr(partial), ptr(dgb), ptr(g_pm), stream_ptr()), "cl3d_bn_relu_bwd")
+    check(L.cl3d_bn_relu_bwd(ptr(grad_y), dt, ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, int(training),
+                             ptr(partial), ptr(dgb), ptr(g_pm), stream_ptr()), "cl3d_bn_relu_bwd")
     return g_pm, dgb[0], dgb[1]
 
 
@@ -321,8 +321,8 @@ def to_point_major_aug(x_cn, xyz, radius):
     dt = require_features(x_cn, "features")
     B, C, N = x_cn.shape
     out = torch.empty(B, N, padded_channels(C + 3), dtype=F32, device=x_cn.device)
-    check(_lib.lib().cl3d_to_point_major_aug_dt(ptr(x_cn), dt, ptr(xyz), B, C, N, float(radius), ptr(out),
-                                                stream_ptr()), "cl3d_to_point_major_aug")
+    check(_lib.lib().cl3d_to_point_major_aug(ptr(x_cn), dt, ptr(xyz), B, C, N, float(radius), ptr(out),
+                                             stream_ptr()), "cl3d_to_point_major_aug")
     return out
 
 
@@ -369,8 +369,8 @@ def pwmlp_fwd_stats(ab_pm, wp, sgn, query_xyz, support_xyz, idx, Cout, radius):
 def pwmlp_fwd_out(ysel, stats, gamma, beta, dtype=F32):
     B, Cout, M = ysel.shape
     out = torch.empty(B, Cout, M, dtype=dtype, device=ysel.device)
-    check(_lib.lib().cl3d_pwmlp_fwd_out_dt(ptr(ysel), ptr(stats), ptr(gamma), ptr(beta), B, M, Cout, ptr(out),
-                                           DTYPE_CODE[dtype], stream_ptr()), "cl3d_pwmlp_fwd_out")
+    check(_lib.lib().cl3d_pwmlp_fwd_out(ptr(ysel), ptr(stats), ptr(gamma), ptr(beta), B, M, Cout, ptr(out),
+                                        DTYPE_CODE[dtype], stream_ptr()), "cl3d_pwmlp_fwd_out")
     return out
 
 
@@ -389,7 +389,7 @@ def pwmlp_bwd(grad_out, beta, ab_pm, wp, sgn, query_xyz, support_xyz, idx, csr_o
     dgb = torch.empty(2, Cout, dtype=F32, device=dev)
     grad_ab = torch.empty(B, N, C2, dtype=F32, device=dev)
     grad_wp = torch.empty(3, Cout, dtype=F32, device=dev)
-    check(L.cl3d_pwmlp_bwd_dt(ptr(grad_out), dt, ptr(beta), ptr(ab_pm), ptr(wp), ptr(sgn), ptr(query_xyz), ptr(support_xyz), ptr(idx),
+    check(L.cl3d_pwmlp_bwd(ptr(grad_out), dt, ptr(beta), ptr(ab_pm), ptr(wp), ptr(sgn), ptr(query_xyz), ptr(support_xyz), ptr(idx),
                            ptr(csr_off), ptr(csr_ent), ptr(ysel), ptr(aq), ptr(sq), ptr(karg), ptr(stats), ptr(gamma),
                            B, N, M, K, Cout, float(radius), int(bool(training)), ptr(partial), ptr(dgb), ptr(grad_ab),
                            ptr(grad_wp),
@@ -429,8 +429,8 @@ def gather_max(features, idx):
     feat_pm = to_point_major(features)
     out = torch.empty(B, C, M, dtype=features.dtype, device=features.device)
     arg = torch.empty(B, M, feat_pm.shape[2], dtype=torch.uint8, device=features.device)
-    check(_lib.lib().cl3d_gather_max_fwd_dt(ptr(feat_pm), ptr(idx), B, N, M, K, C, ptr(out), dt, ptr(arg),
-                                            stream_ptr()), "cl3d_gather_max_fwd")
+    check(_lib.lib().cl3d_gather_max_fwd(ptr(feat_pm), ptr(idx), B, N, M, K, C, ptr(out), dt, ptr(arg),
+                                         stream_ptr()), "cl3d_gather_max_fwd")
     return out, arg
 
 
@@ -441,8 +441,8 @@ def gather_max_grad(grad_out, idx, arg, N):
     B, C, M = grad_out.shape
     K = idx.shape[2]
     g_pm = torch.empty(B, N, padded_channels(C), dtype=F32, device=grad_out.device)
-    check(_lib.lib().cl3d_gather_max_bwd_dt(ptr(grad_out), dt, ptr(idx), ptr(arg), B, N, M, K, C, ptr(g_pm),
-                                            stream_ptr()), "cl3d_gather_max_bwd")
+    check(_lib.lib().cl3d_gather_max_bwd(ptr(grad_out), dt, ptr(idx), ptr(arg), B, N, M, K, C, ptr(g_pm),
+                                         stream_ptr()), "cl3d_gather_max_bwd")
     return to_channel_major(g_pm, C, grad_out.dtype)
 
 

@@ -4,7 +4,7 @@ signatures, return shapes and autograd behaviour, running on libcl3d's sm_90a ke
 
     reference name (pt_utils.py line)            here
     grouping_operation            (:64)          GroupingOperation.apply      -> cl3d_group_points[_grad]
-    masked_ordered_ball_query     (:80)          MaskedOrderedBallQuery.apply -> cl3d_ball_query (grid hash)
+    masked_ordered_ball_query     (:80)          MaskedOrderedBallQuery.apply -> cl3d_ball_query_algo (grid hash)
     masked_nearest_query          (:95)          MaskedNearestQuery.apply     -> cl3d_nearest_query
     masked_grid_subsampling       (:111)         MaskedGridSubsampling.apply  -> cl3d_grid_subsample
     MaskedQueryAndGroup           (:114)         same forward contract (materialising compat path)

@@ -51,10 +51,10 @@ extern "C" {
 #define CL3D_FAM_ADAPTIVE_DP 2    /* AdaptiveWeight, weight_type='dp', num_mlps=1 (:188-197) */
 #define CL3D_FAM_PSEUDOGRID 3     /* PseudoGrid, linear / constant influence, sum (:368-419) */
 
-/* Element type of a channel-major feature tensor (the `_dt` entry points below).  Only the tensors that cross the
- * channel-major <-> point-major boundary take it; inside, every buffer and every operation stays fp32.  A 16-bit
- * input is widened exactly; an fp32 result is rounded once, to nearest even, where it is stored.  Unknown codes:
- * CL3D_ERR_BAD_ARG.  Each fp32 entry point is its `_dt` twin with CL3D_DTYPE_F32. */
+/* Element type of a channel-major feature tensor: an entry point that reads or writes one takes it as `int dtype`
+ * beside the pointer it describes (`const void*` / `void*`).  Only the tensors that cross the channel-major <->
+ * point-major boundary take it; inside, every buffer and every operation stays fp32.  A 16-bit input is widened
+ * exactly; an fp32 result is rounded once, to nearest even, where it is stored.  Unknown codes: CL3D_ERR_BAD_ARG. */
 #define CL3D_DTYPE_F32 0
 #define CL3D_DTYPE_F16 1
 #define CL3D_DTYPE_BF16 2
@@ -85,11 +85,8 @@ long long cl3d_launch_count(void);
  * fallback when a neighbourhood overflows the on-chip candidate list.
  * ---------------------------------------------------------------------------------------------- */
 size_t cl3d_ball_query_workspace_bytes(int B, int N, int M, int K);
-int cl3d_ball_query(const float* query_xyz, const float* support_xyz, const int* query_mask,
-                    const int* support_mask, int B, int N, int M, float radius, int K, int* idx,
-                    int* idx_mask, int* ncount, void* workspace, size_t workspace_bytes,
-                    cl3d_stream_t stream);
-/* same, with the search algorithm forced (tests / benchmarks): AUTO picks brute force for N <= 2048 */
+/* algo: CL3D_BQ_AUTO picks brute force for N <= 2048 and the grid otherwise; BRUTE / GRID force one (tests,
+ * benchmarks) */
 #define CL3D_BQ_AUTO 0
 #define CL3D_BQ_BRUTE 1
 #define CL3D_BQ_GRID 2
@@ -135,19 +132,15 @@ int cl3d_build_csr(const int* idx, const int* ncount, int B, int N, int M, int K
  * Compatibility gather / scatter (the reference's materialising path; kept for the non-fused module API).
  * Replace _ext.group_points / _ext.group_points_grad (group_points_gpu.cu:13-33,48-69).
  * ---------------------------------------------------------------------------------------------- */
-int cl3d_group_points(const float* points /*(B,C,N)*/, const int* idx /*(B,M,K)*/, int B, int C, int N,
-                      int M, int K, float* out /*(B,C,M,K)*/, cl3d_stream_t stream);
-/* grad_points (B,C,N) is fully overwritten (zero-filled first); contributions are added with fp32 atomics, so the
- * summation order -- like the reference's group_points_grad_gpu.cu:48-69 -- is not deterministic (tolerance parity). */
-int cl3d_group_points_grad(const float* grad_out /*(B,C,M,K)*/, const int* idx, int B, int C, int N,
-                           int M, int K, float* grad_points, cl3d_stream_t stream);
-/* points / out and grad_out / grad_points in `dtype`.  The 16-bit gradient is accumulated with fp32 atomics into
- * `acc` (B*C*N floats of caller scratch; may be NULL for CL3D_DTYPE_F32, which accumulates in grad_points) and
- * converted once. */
-int cl3d_group_points_dt(const void* points, int dtype, const int* idx, int B, int C, int N, int M, int K, void* out,
-                         cl3d_stream_t stream);
-int cl3d_group_points_grad_dt(const void* grad_out, int dtype, const int* idx, int B, int C, int N, int M, int K,
-                              void* grad_points, float* acc, cl3d_stream_t stream);
+/* points / out and grad_out / grad_points in `dtype`.
+ * grad_points (B,C,N) is fully overwritten (zero-filled first); contributions are added with fp32 atomics, so the
+ * summation order -- like the reference's group_points_grad_gpu.cu:48-69 -- is not deterministic (tolerance parity).
+ * A 16-bit gradient is accumulated into `acc` (B*C*N floats of caller scratch; may be NULL for CL3D_DTYPE_F32, which
+ * accumulates in grad_points) and converted once. */
+int cl3d_group_points(const void* points /*(B,C,N)*/, int dtype, const int* idx /*(B,M,K)*/, int B, int C, int N,
+                      int M, int K, void* out /*(B,C,M,K)*/, cl3d_stream_t stream);
+int cl3d_group_points_grad(const void* grad_out /*(B,C,M,K)*/, int dtype, const int* idx, int B, int C, int N,
+                           int M, int K, void* grad_points, float* acc, cl3d_stream_t stream);
 
 /* Replaces _ext.masked_grid_subsampling (masked_grid_subsampling_gpu.cu:11-153).
  * sub_xyz (B,m,3) f32, sub_mask (B,m) i32. */
@@ -158,25 +151,19 @@ int cl3d_grid_subsample(const float* points, const int* mask, int B, int n, int 
 
 /* Fused neighbourhood max-pool (body of MaskedMaxPool, pt_utils.py:195-201) and its gradient.
  *   feat_pm (B,N,Cp) point-major (+CL3D_PM_SLACK); out (B,C,M); arg (B,M,Cp) uint8 first arg-max slot (K <= 255)
- *   bwd: grad_pm (B,N,Cp) point-major, zero-filled by the call then accumulated (one red.add row per query). */
-int cl3d_gather_max_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, float* out,
-                        unsigned char* arg, cl3d_stream_t stream);
-int cl3d_gather_max_bwd(const float* grad_out, const int* idx, const unsigned char* arg, int B, int N, int M,
-                        int K, int C, float* grad_pm, cl3d_stream_t stream);
-/* out / grad_out in `dtype` (the maximum of exactly widened values is exact); feat_pm, grad_pm fp32 */
-int cl3d_gather_max_fwd_dt(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, void* out,
-                           int dtype, unsigned char* arg, cl3d_stream_t stream);
-int cl3d_gather_max_bwd_dt(const void* grad_out, int dtype, const int* idx, const unsigned char* arg, int B, int N,
-                           int M, int K, int C, float* grad_pm, cl3d_stream_t stream);
+ *   bwd: grad_pm (B,N,Cp) point-major, zero-filled by the call then accumulated (one red.add row per query).
+ *   out / grad_out in `dtype` (the maximum of exactly widened values is exact); feat_pm, grad_pm fp32. */
+int cl3d_gather_max_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, void* out,
+                        int dtype, unsigned char* arg, cl3d_stream_t stream);
+int cl3d_gather_max_bwd(const void* grad_out, int dtype, const int* idx, const unsigned char* arg, int B, int N,
+                        int M, int K, int C, float* grad_pm, cl3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Layout: channel-major (B,C,N) <-> point-major (B,N,Cp), Cp = cl3d_padded_channels(C), pad = 0.
+ * The channel-major side in `dtype`; the point-major side fp32.
  * ---------------------------------------------------------------------------------------------- */
-int cl3d_to_point_major(const float* in_cn, int B, int C, int N, float* out_nc, cl3d_stream_t stream);
-int cl3d_to_channel_major(const float* in_nc, int B, int C, int N, float* out_cn, cl3d_stream_t stream);
-/* the channel-major side in `dtype`; the point-major side fp32 */
-int cl3d_to_point_major_dt(const void* in_cn, int dtype, int B, int C, int N, float* out_nc, cl3d_stream_t stream);
-int cl3d_to_channel_major_dt(const float* in_nc, int B, int C, int N, void* out_cn, int dtype, cl3d_stream_t stream);
+int cl3d_to_point_major(const void* in_cn, int dtype, int B, int C, int N, float* out_nc, cl3d_stream_t stream);
+int cl3d_to_channel_major(const float* in_nc, int B, int C, int N, void* out_cn, int dtype, cl3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused aggregation, families PosPool(xyz|sin_cos) / AdaptiveWeight(dp) / PseudoGrid.
@@ -195,7 +182,7 @@ int cl3d_to_channel_major_dt(const float* in_nc, int B, int C, int N, void* out_
  *               ntiles = cl3d_agg_num_tiles(B,M).  May be NULL.
  * backward (gather form over the CSR lists; no float atomics on activations):
  *   g_pm      (B,M,Cp) point-major d(loss)/d(agg)
- *   grad_feat (B,C,N) channel-major out, fully written
+ *   grad_feat (B,C,N) channel-major out in `dtype`, fully written (by each backward kernel's own channel-major store)
  *   grad_params_partial (nblocks, P) out: per-CTA partial parameter gradients, nblocks =
  *               cl3d_agg_bwd_num_blocks(B,N), P = cl3d_agg_num_params(...) laid out (slot, C) with
  *               slot = {x,y,z,bias} (ADAPTIVE_DP, per channel: the caller folds `shared` groups) or the
@@ -217,15 +204,8 @@ int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const float* feat
                  const float* query_xyz, const float* support_xyz, const int* ncount,
                  const int* csr_off, const int* csr_ent, const float* p0, const float* p1, int B, int N,
                  int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
-                 int influence, float* grad_feat, float* grad_params_partial,
+                 int influence, void* grad_feat, int dtype, float* grad_params_partial,
                  const unsigned char* arg_pm, cl3d_stream_t stream);
-/* grad_feat written in `dtype` (by each backward kernel's own channel-major store); everything else as above */
-int cl3d_agg_bwd_dt(int family, int reduction, const float* g_pm, const float* feat_pm,
-                    const float* query_xyz, const float* support_xyz, const int* ncount,
-                    const int* csr_off, const int* csr_ent, const float* p0, const float* p1, int B, int N,
-                    int M, int K, int C, float radius, int normalize, int shared, int nkp, float extent,
-                    int influence, void* grad_feat, int dtype, float* grad_params_partial,
-                    const unsigned char* arg_pm, cl3d_stream_t stream);
 /* out[p] = sum_t partial[t][p]  (fixed order -> deterministic given the partials) */
 int cl3d_reduce_partials(const float* partial, int ntiles, int P, float* out, cl3d_stream_t stream);
 
@@ -236,21 +216,16 @@ int cl3d_reduce_partials(const float* partial, int ntiles, int P, float* out, cl
  *   bn_relu_fwd: y = relu((x-mean)*invstd*gamma + beta); in eval mode pass stats made from running stats.
  *   bn_relu_bwd_stats / bn_relu_bwd_apply: two-phase backward; apply writes d(loss)/d(agg) POINT-MAJOR
  *                (B,M,Cp) ready for cl3d_agg_bwd, and dgamma/dbeta.
+ *   y written / grad_y read in `dtype`; x, the statistics, partials, dgamma_dbeta and g_pm fp32.
  * ---------------------------------------------------------------------------------------------- */
 int cl3d_bn_finalize(const float* bn_partial, int ntiles, int C, long long count, float eps,
                      float momentum, int training, float* running_mean, float* running_var,
                      float* save_stats /*(2,C): mean, invstd*/, cl3d_stream_t stream);
 int cl3d_bn_relu_fwd(const float* x, const float* save_stats, const float* gamma, const float* beta,
-                     int B, int C, int M, float* y, cl3d_stream_t stream);
-int cl3d_bn_relu_bwd(const float* grad_y, const float* x, const float* save_stats, const float* gamma,
+                     int B, int C, int M, void* y, int dtype, cl3d_stream_t stream);
+int cl3d_bn_relu_bwd(const void* grad_y, int dtype, const float* x, const float* save_stats, const float* gamma,
                      const float* beta, int B, int C, int M, int training, float* partial /*(ntiles,2,C)*/,
                      float* dgamma_dbeta /*(2,C)*/, float* g_pm /*(B,M,Cp)*/, cl3d_stream_t stream);
-/* y written / grad_y read in `dtype`; x, the statistics, partials, dgamma_dbeta and g_pm fp32 */
-int cl3d_bn_relu_fwd_dt(const float* x, const float* save_stats, const float* gamma, const float* beta,
-                        int B, int C, int M, void* y, int dtype, cl3d_stream_t stream);
-int cl3d_bn_relu_bwd_dt(const void* grad_y, int dtype, const float* x, const float* save_stats, const float* gamma,
-                        const float* beta, int B, int C, int M, int training, float* partial,
-                        float* dgamma_dbeta, float* g_pm, cl3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused PointWiseMLP (feature_type='dp_fi_df', num_mlps=1, reduction='max';
@@ -264,28 +239,29 @@ int cl3d_bn_relu_bwd_dt(const void* grad_y, int dtype, const float* x, const flo
  *   C[m][n] = sum_k A[m*sa_m + k*sa_k] * B[k*sb_k + n*sb_n],  C row stride ldc.
  * splitk > 1 divides k among CTAs (fixed-order reduction); workspace = cl3d_sgemm_workspace_bytes.
  * algo: CL3D_GEMM_TC3X = wgmma tensor cores with the 3xTF32 operand split (fp32-level accuracy, the default
- * behind CL3D_GEMM_AUTO), CL3D_GEMM_FFMA = fp32 FMA pipe.  cl3d_sgemm == cl3d_sgemm_algo(..., CL3D_GEMM_AUTO). */
+ * behind CL3D_GEMM_AUTO), CL3D_GEMM_FFMA = fp32 FMA pipe. */
 #define CL3D_GEMM_AUTO 0
 #define CL3D_GEMM_FFMA 1
 #define CL3D_GEMM_TC3X 2
 size_t cl3d_sgemm_workspace_bytes(int M, int N, int splitk);
-int cl3d_sgemm(const float* a, long long sa_m, long long sa_k, const float* b, long long sb_k,
-               long long sb_n, int M, int N, int K, float* c, long long ldc, int splitk, void* workspace,
-               size_t workspace_bytes, cl3d_stream_t stream);
 int cl3d_sgemm_algo(const float* a, long long sa_m, long long sa_k, const float* b, long long sb_k,
                     long long sb_n, int M, int N, int K, float* c, long long ldc, int splitk, void* workspace,
                     size_t workspace_bytes, int algo, cl3d_stream_t stream);
 
 /* Fused PointWiseMLP (pwmlp.cu).  Cop = cl3d_padded_channels(Cout), Cpa = cl3d_padded_channels(C+3).
- *   cl3d_to_point_major_aug : (B,C,N) features + (B,N,3) xyz -> (B,N,Cpa) rows [f | (xyz - o_b)/r | 0], o_b = xyz[b,0]
+ *   cl3d_to_point_major_aug : (B,C,N) features in `dtype` + (B,N,3) xyz -> (B,N,Cpa) fp32 rows
+ *                             [f | (xyz - o_b)/r | 0], o_b = xyz[b,0]
  *                             (support_xyz of fwd_stats / bwd supplies the same origin for the query term)
- *   ab_pm (B,N,2*Cop)       : row = [A | T],  A = (Wc-Wr) f,  T = sgn*(Wr f + Wp s/r)   (one cl3d_sgemm)
+ *   ab_pm (B,N,2*Cop)       : row = [A | T],  A = (Wc-Wr) f,  T = sgn*(Wr f + Wp s/r)   (one cl3d_sgemm_algo)
  *   wp (Cout,3), sgn (Cout) : conv weight columns 0..2; sign(gamma) as +-1.0
  * fwd_stats : ysel (B,Cout,M) selected extremum of y; aq, sq (B,M,Cop) a' and sum_k bv; karg (B,M,Cop) uint8
  *             first arg-max slot (K <= 255); bn_partial (cl3d_agg_num_tiles(B,M), 2, Cout) -> cl3d_bn_finalize
  *             with count = B*M*K.
- * fwd_out   : out (B,Cout,M) = relu(sc*ysel + sh).
- * bwd       : csr_off/csr_ent = cl3d_build_csr over ALL K slots (ncount = K); scratch =
+ * fwd_out   : out (B,Cout,M) = relu(sc*ysel + sh), in `dtype`.
+ * bwd       : grad_out (B,Cout,M) in `dtype`.  The ReLU decision is recomputed from ysel, save_stats, gamma and beta
+ *             with the forward's expression (bit-identical to the forward's fp32 decision; a 16-bit output may have
+ *             rounded a small positive value to zero, so the stored output cannot decide).
+ *             csr_off/csr_ent = cl3d_build_csr over ALL K slots (ncount = K); scratch =
  *             cl3d_pwmlp_bwd_scratch_floats(...) floats; dgamma_dbeta (2,Cout); grad_ab_pm (B,N,2*Cop) fully
  *             written (zero-filled, then the support-major pass and the query pass add their parts with fp32
  *             red.add); side_stream (may be NULL): the zero-fill and the query pass run on it beside the other
@@ -300,33 +276,20 @@ int cl3d_pwmlp_prep_weights(const float* conv_weight, const float* gamma, int C,
                             float* wp, float* sgn, cl3d_stream_t stream);
 int cl3d_pwmlp_weight_grad(const float* gwcat, const float* grad_wp, const float* sgn, int C, int Cout,
                            float* grad_conv_weight, cl3d_stream_t stream);
-int cl3d_to_point_major_aug(const float* in_cn, const float* xyz, int B, int C, int N, float radius,
+int cl3d_to_point_major_aug(const void* in_cn, int dtype, const float* xyz, int B, int C, int N, float radius,
                             float* out_nc, cl3d_stream_t stream);
 int cl3d_pwmlp_fwd_stats(const float* ab_pm, const float* wp, const float* sgn, const float* query_xyz,
                          const float* support_xyz, const int* idx, int B, int N, int M, int K, int Cout,
                          float radius, float* ysel,
                          float* aq, float* sq, unsigned char* karg, float* bn_partial, cl3d_stream_t stream);
 int cl3d_pwmlp_fwd_out(const float* ysel, const float* save_stats, const float* gamma, const float* beta,
-                       int B, int M, int Cout, float* out, cl3d_stream_t stream);
-int cl3d_pwmlp_bwd(const float* grad_out, const float* out, const float* ab_pm, const float* wp,
+                       int B, int M, int Cout, void* out, int dtype, cl3d_stream_t stream);
+int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta, const float* ab_pm, const float* wp,
                    const float* sgn, const float* query_xyz, const float* support_xyz, const int* idx,
                    const int* csr_off, const int* csr_ent, const float* ysel, const float* aq, const float* sq,
                    const unsigned char* karg, const float* save_stats, const float* gamma, int B, int N,
                    int M, int K, int Cout, float radius, int training, float* scratch, float* dgamma_dbeta,
                    float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream, cl3d_stream_t side_stream);
-/* in_cn / out / grad_out in `dtype`.  cl3d_pwmlp_bwd_dt takes beta instead of the stored output: the ReLU decision
- * is recomputed from ysel, save_stats, gamma and beta with the forward's expression (bit-identical to the forward's
- * fp32 decision; a 16-bit output may have rounded a small positive value to zero). */
-int cl3d_to_point_major_aug_dt(const void* in_cn, int dtype, const float* xyz, int B, int C, int N, float radius,
-                               float* out_nc, cl3d_stream_t stream);
-int cl3d_pwmlp_fwd_out_dt(const float* ysel, const float* save_stats, const float* gamma, const float* beta,
-                          int B, int M, int Cout, void* out, int dtype, cl3d_stream_t stream);
-int cl3d_pwmlp_bwd_dt(const void* grad_out, int dtype, const float* beta, const float* ab_pm, const float* wp,
-                      const float* sgn, const float* query_xyz, const float* support_xyz, const int* idx,
-                      const int* csr_off, const int* csr_ent, const float* ysel, const float* aq, const float* sq,
-                      const unsigned char* karg, const float* save_stats, const float* gamma, int B, int N,
-                      int M, int K, int Cout, float radius, int training, float* scratch, float* dgamma_dbeta,
-                      float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream, cl3d_stream_t side_stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused multi-shape part-segmentation head (multihead.cu).  Replaces the S per-shape heads of

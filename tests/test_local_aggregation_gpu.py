@@ -5,6 +5,8 @@ Tolerance (BASELINE.json north_star): fp32 outputs within 1e-5 of the reference 
 relative to their max magnitude.  Neighbour indices are compared bit-exact in test_neighbors_gpu.py.
 """
 import copy
+import os
+import re
 
 import pytest
 import torch
@@ -204,3 +206,34 @@ def test_composed_settings(cuda, oracle_ext, la_type, over):
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     run_case(cuda, oracle_ext, la_type, over, 2, 600, 12, 36, seed=5, tol=2e-5)
+
+
+def _declared_functions():
+    with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "cl3d.h")) as fh:
+        hdr = fh.read()
+    return set(re.findall(r"\b(cl3d_[a-z0-9_]+)\s*\(", re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)))
+
+
+@pytest.mark.parametrize("la_type,over,entries", [
+    ("pseudo_grid", dict(), {"cl3d_to_point_major", "cl3d_agg_fwd", "cl3d_agg_bwd", "cl3d_bn_relu_fwd",
+                             "cl3d_bn_relu_bwd"}),
+    ("pointwisemlp", PW, {"cl3d_sgemm_algo", "cl3d_pwmlp_fwd_stats", "cl3d_pwmlp_fwd_out", "cl3d_pwmlp_bwd",
+                          "cl3d_to_channel_major"}),
+])
+def test_profiler_records_declared_entry_points(cuda, la_type, over, entries):
+    # bench.py's kernel model and tools/bench_pg.py look the profiler's records up by the names include/cl3d.h declares
+    from closerlook3d_b200 import _lib
+    from closerlook3d_b200.local_aggregation_operators import LocalAggregation
+    B, N, K, C = 2, 1024, 16, 72
+    torch.manual_seed(0)
+    mod = LocalAggregation(C, C, synth.ball_radius(N, K), K, la_config(la_type, **over)).to(cuda)
+    d = synth.make_cloud_batch(B, N, C, 0)
+    xyz, mask = d["xyz"].to(cuda), d["mask"].to(cuda)
+    f = d["features"].to(cuda).requires_grad_(True)
+    _lib.profiler.start()
+    try:
+        mod(xyz, xyz, mask, mask, f).sum().backward()
+    finally:
+        recorded = set(_lib.profiler.stop())
+    assert recorded <= _declared_functions(), f"recorded but not declared: {sorted(recorded - _declared_functions())}"
+    assert entries <= recorded, f"not recorded: {sorted(entries - recorded)}"

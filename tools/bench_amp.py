@@ -4,8 +4,8 @@ alternated, CUDA events per step and per libcl3d entry point.
 
     python tools/bench_amp.py [--configs 3 5] [--steps 30] [--rounds 5]
 
-Arms: fp32 (features float32); bf16 (bfloat16 features through the _dt entry points); B (the fp32 operator behind
-explicit .float() / .to(bfloat16) conversions: what a caller without native 16-bit support would run).
+Arms: fp32 (features float32); bf16 (bfloat16 features through the entry points' dtype arguments); B (the fp32
+operator behind explicit .float() / .to(bfloat16) conversions: what a caller without native 16-bit support would run).
 c3 = PseudoGrid linear, B 8, N 15000, K 26, C 72; c5 = PosPool sin_cos avg, B 8 (one GPU's shard), N 40000, K 40,
 C 144 (BASELINE.md).  Prints one JSON line per (config, arm): ms per step, median [min..max] over the rounds, and
 the median ms per entry point; then the card, its power limit and SM clock.
