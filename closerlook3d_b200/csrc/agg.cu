@@ -305,7 +305,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, FAM == CL3D_FAM_PSEUDOGRID ? 2
     for (int i = 0; i < CI; ++i) s_out[(size_t)(lane + 32 * i) * (kTile + 1) + ql] = res[i];
   }
   __syncthreads();
-  // ---- write the tile channel-major + BatchNorm partial sums (one warp per channel row)
+  // ---- write the tile channel-major + BatchNorm partial moments (one warp per channel row)
   const int q = q0 + lane;
   for (int cl = warp; cl < 32 * CI; cl += kAggWarps) {
     const int c = c0 + cl;
@@ -315,13 +315,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, FAM == CL3D_FAM_PSEUDOGRID ? 2
       v = s_out[(size_t)cl * (kTile + 1) + lane];
       a.out[((size_t)b * a.C + c) * a.M + q] = v;
     }
-    if (a.partial) {
-      const float s1 = warp_sum(v), s2 = warp_sum(v * v);
-      if (lane == 0) {
-        a.partial[((size_t)blockIdx.x * 2 + 0) * a.C + c] = s1;
-        a.partial[((size_t)blockIdx.x * 2 + 1) * a.C + c] = s2;
-      }
-    }
+    if (a.partial) warp_bn_moments(a.partial, blockIdx.x, a.C, c, v, q < a.M);
   }
 }
 
@@ -742,13 +736,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, 3) sincos_fwd_kernel(const Agg
       v = s_out[(size_t)r * (kTile + 1) + lane];
       a.out[((size_t)b * a.C + c) * a.M + q] = v;
     }
-    if (a.partial) {
-      const float s1 = warp_sum(v), s2 = warp_sum(v * v);
-      if (lane == 0) {
-        a.partial[((size_t)blockIdx.x * 2 + 0) * a.C + c] = s1;
-        a.partial[((size_t)blockIdx.x * 2 + 1) * a.C + c] = s2;
-      }
-    }
+    if (a.partial) warp_bn_moments(a.partial, blockIdx.x, a.C, c, v, q < a.M);
   }
 }
 

@@ -82,7 +82,7 @@ __global__ void __launch_bounds__(kAggWarps * 32) aggmax_fwd_kernel(const AggArg
     for (int i = 0; i < CI; ++i) s_out[lane + 32 * i][ql] = best[i];
   }
   __syncthreads();
-  // ---- the tile channel-major + BatchNorm partial sums (one warp per channel row), as agg_fwd_kernel
+  // ---- the tile channel-major + BatchNorm partial moments (one warp per channel row), as agg_fwd_kernel
   const int q = q0 + lane;
   for (int cl = warp; cl < 32 * CI; cl += kAggWarps) {
     const int c = c0 + cl;
@@ -92,13 +92,7 @@ __global__ void __launch_bounds__(kAggWarps * 32) aggmax_fwd_kernel(const AggArg
       v = s_out[cl][lane];
       a.out[((size_t)b * a.C + c) * a.M + q] = v;
     }
-    if (a.partial) {
-      const float s1 = warp_sum(v), s2 = warp_sum(v * v);
-      if (lane == 0) {
-        a.partial[((size_t)blockIdx.x * 2 + 0) * a.C + c] = s1;
-        a.partial[((size_t)blockIdx.x * 2 + 1) * a.C + c] = s2;
-      }
-    }
+    if (a.partial) warp_bn_moments(a.partial, blockIdx.x, a.C, c, v, q < a.M);
   }
 }
 

@@ -3,7 +3,7 @@
 //
 // Replaces nn.Sequential(nn.BatchNorm1d(C, momentum), nn.ReLU(inplace=True)) of
 //   /root/reference/pytorch/models/local_aggregation_operators.py:43-45,110 (and :166-168, :363-365).
-// Batch statistics come from the per-tile partial sums the aggregation kernel already produced, so the
+// Batch statistics come from the per-tile moments the aggregation kernel already produced, so the
 // forward costs one read + one write of (B,C,M); the backward is two passes (statistics, apply) and writes
 // d(loss)/d(agg) directly in the point-major layout the gather-form aggregation backward consumes.
 #include <type_traits>
@@ -14,8 +14,17 @@ namespace cl3d {
 
 constexpr int kBnTile = 32;
 
-// mean / invstd from the partial sums; running-stat update as nn.BatchNorm1d (unbiased variance).
-// One CTA of 1024 threads handles 32 channels (32 tile-lanes each), deterministic.
+// one tile's moments (store_bn_moments) added to the sums of (x - shift) and (x - shift)^2: with g = centre - shift,
+//   sum (x - shift) = d + n g,   sum (x - shift)^2 = q + 2 g d + n g^2
+__device__ __forceinline__ void bn_tile_add(const float* __restrict__ p, int C, double shift, double& a1, double& a2) {
+  const double n = p[0], g = (double)p[C] - shift, d = p[2 * C], q = p[3 * C];
+  a1 += fma(n, g, d);
+  a2 += fma(g, fma(n, g, 2.0 * d), q);
+}
+
+// mean / invstd from the per-tile moments; running-stat update as nn.BatchNorm1d (unbiased variance).
+// The tiles are merged in double about one shift per channel, tile 0's centre (a value of the channel, so the sums
+// are of spread-sized terms and the variance never cancels against the mean), in a fixed order: deterministic.
 // One CTA = 8 channels (one 32-byte sector of a partial row) x 128 tile slices: C/8 CTAs, so the whole partial
 // array is in flight at once (the kernel sits on the forward's critical path and is pure load latency).
 __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restrict__ partial, int ntiles, int C,
@@ -26,24 +35,20 @@ __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restri
   __shared__ double s1[128][9], s2[128][9];
   const int tx = threadIdx.x & 7, ty = threadIdx.x >> 3;
   const int c = blockIdx.x * 8 + tx;
+  const size_t ts = (size_t)kBnRows * C;  // floats per tile
+  const double shift = training && c < C ? (double)partial[C + c] : 0.0;
   double a1 = 0.0, a2 = 0.0;
   if (training && c < C) {
+    const float* p = partial + c;
     double b1 = 0.0, b2 = 0.0, c1 = 0.0, c2 = 0.0, d1 = 0.0, d2 = 0.0;
     int t = ty;
     for (; t + 384 < ntiles; t += 512) {  // four independent load streams per thread
-      a1 += (double)partial[((size_t)t * 2 + 0) * C + c];
-      a2 += (double)partial[((size_t)t * 2 + 1) * C + c];
-      b1 += (double)partial[((size_t)(t + 128) * 2 + 0) * C + c];
-      b2 += (double)partial[((size_t)(t + 128) * 2 + 1) * C + c];
-      c1 += (double)partial[((size_t)(t + 256) * 2 + 0) * C + c];
-      c2 += (double)partial[((size_t)(t + 256) * 2 + 1) * C + c];
-      d1 += (double)partial[((size_t)(t + 384) * 2 + 0) * C + c];
-      d2 += (double)partial[((size_t)(t + 384) * 2 + 1) * C + c];
+      bn_tile_add(p + (size_t)t * ts, C, shift, a1, a2);
+      bn_tile_add(p + (size_t)(t + 128) * ts, C, shift, b1, b2);
+      bn_tile_add(p + (size_t)(t + 256) * ts, C, shift, c1, c2);
+      bn_tile_add(p + (size_t)(t + 384) * ts, C, shift, d1, d2);
     }
-    for (; t < ntiles; t += 128) {
-      a1 += (double)partial[((size_t)t * 2 + 0) * C + c];
-      a2 += (double)partial[((size_t)t * 2 + 1) * C + c];
-    }
+    for (; t < ntiles; t += 128) bn_tile_add(p + (size_t)t * ts, C, shift, a1, a2);
     a1 = (a1 + b1) + (c1 + d1);
     a2 = (a2 + b2) + (c2 + d2);
   }
@@ -60,9 +65,9 @@ __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restri
   }
   if (ty == 0 && c < C) {
     if (training) {
-      const double sum = s1[0][tx], sq = s2[0][tx];
-      const double mean = sum / count;
-      double var = sq / count - mean * mean;
+      const double dm = s1[0][tx] / count;  // mean - shift
+      const double mean = shift + dm;
+      double var = s2[0][tx] / count - dm * dm;
       if (var < 0.0) var = 0.0;
       save_stats[c] = (float)mean;
       save_stats[C + c] = (float)(1.0 / sqrt(var + (double)eps));
@@ -252,7 +257,7 @@ extern "C" int cl3d_bn_finalize(const float* bn_partial, int ntiles, int C, long
                                 int training, float* running_mean, float* running_var, float* save_stats,
                                 cl3d_stream_t stream_) {
   CL3D_REQUIRE(C >= 1 && save_stats, "cl3d_bn_finalize: bad arguments");
-  CL3D_REQUIRE(!training || (bn_partial && ntiles >= 1 && count >= 1), "cl3d_bn_finalize: training needs partial sums");
+  CL3D_REQUIRE(!training || (bn_partial && ntiles >= 1 && count >= 1), "cl3d_bn_finalize: training needs partial moments");
   CL3D_REQUIRE(training || (running_mean && running_var), "cl3d_bn_finalize: eval needs running statistics");
   bn_finalize_kernel<<<ceil_div(C, 8), 1024, 0, (cudaStream_t)stream_>>>(bn_partial, ntiles, C, (double)count, eps,
                                                                          momentum, training, running_mean,

@@ -127,6 +127,47 @@ __device__ __forceinline__ int warp_sum_i(int v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+
+// ---- BatchNorm forward partials: (ntiles, kBnRows, C), one row group per tile, tiles of one cloud contiguous.
+// Per tile and channel: [0] n, the number of values; [1] c, a centre near the tile's values; [2] sum (x - c);
+// [3] sum (x - c)^2.  The sums are of small, spread-sized terms, so a channel whose mean dwarfs its spread keeps its
+// variance: a raw fp32 sum of squares loses (mean/std)^2 * 2^-24 of it, a raw fp32 tile sum ~ 2^-24 * |mean| of the
+// tile mean, and both cancel in the finalize.  cl3d_bn_finalize merges the tiles in double.
+constexpr int kBnRows = CL3D_BN_PARTIAL_ROWS;
+
+__device__ __forceinline__ void store_bn_moments(float* partial, size_t tile, int C, int c, float n, float ctr,
+                                                 float d, float q) {
+  float* p = partial + tile * kBnRows * C + c;
+  p[0] = n;
+  p[C] = ctr;
+  p[2 * C] = d;
+  p[3 * C] = q;
+}
+
+// one tile row held one value per lane (queries q0 + lane, present where q < M; lane 0 always is), centred about its
+// fp32 mean (a centre at one of the values would make sum (x - c)^2 cancel when that value is an outlier, e.g. a
+// padded query); absent lanes count nothing
+__device__ __forceinline__ void warp_bn_moments(float* partial, size_t tile, int C, int c, float v, bool present) {
+  const int n = __popc(__ballot_sync(0xffffffffu, present));
+  const float ctr = __fdividef(warp_sum(present ? v : 0.f), (float)n);  // any centre near the values will do
+  const float e = present ? __fsub_rn(v, ctr) : 0.f;
+  const float d = warp_sum(e), q = warp_sum(e * e);
+  if ((threadIdx.x & 31) == 0) store_bn_moments(partial, tile, C, c, (float)n, ctr, d, q);
+}
+
+// one tile row of n >= 1 values in shared memory, in order, centred about its fp32 mean
+__device__ __forceinline__ void row_bn_moments(float* partial, size_t tile, int C, int c, const float* row, int n) {
+  float s = 0.f;
+  for (int i = 0; i < n; ++i) s += row[i];
+  const float ctr = __fdividef(s, (float)n);
+  float d = 0.f, q = 0.f;
+  for (int i = 0; i < n; ++i) {
+    const float e = __fsub_rn(row[i], ctr);
+    d += e;
+    q = fmaf(e, e, q);
+  }
+  store_bn_moments(partial, tile, C, c, (float)n, ctr, d, q);
+}
 __device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {

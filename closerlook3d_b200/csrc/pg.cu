@@ -21,7 +21,7 @@
 //     {8-byte entry load, 16-byte weight load, 4 FFMA, branch}: 7 instructions instead of 15;
 //   * influences are evaluated straight-line and packed (two kernel points per instruction), the square root with
 //     the hardware approximation (2^-22 relative: h moves by < 3e-7, far inside the 1e-5 parity bar);
-//   * BatchNorm partial sums are accumulated per lane in registers and combined once per tile;
+//   * BatchNorm partial moments are taken once per tile from the output tile in shared memory;
 //   * the backward uses the same one-accumulator w-form for d/df and adds d/dWk into a per-warp shared-memory
 //     accumulator addressed by the entry's offset: ~64 registers instead of 127.
 // One warp per centre point, 32 centre points per CTA tile; the backward is a persistent tile loop.
@@ -48,7 +48,6 @@ constexpr int kEntStride = kMaxKP + 1;
 //   per warp:  s_rec [32] uint2    {row element offset, number of entries} of the staged neighbours (compacted)
 //              s_ent [32][17] float2  their entries {h, byte offset of the kernel point's weight row}
 //   s_out            [CpR][kPgTile + 1]   output tile (transposed write-out)
-//   s_bn             [warps][2][CpR]      forward: per-warp BatchNorm sums
 //   bwd, per warp:   s_pacc [16][CpR]     d/dWk accumulator (same row layout as s_wk: one offset serves both)
 struct PgSmem {
   size_t kp_off, wk_off, rec_off, ent_off, out_off, aux_off, total;
@@ -70,7 +69,7 @@ __host__ __device__ inline PgSmem pg_smem(int Cp, bool bwd) {
   o += (size_t)L.CpR * (kPgTile + 1) * sizeof(float);
   o = align_up(o, 16);
   L.aux_off = o;
-  o += bwd ? (size_t)kPgWarps * kMaxKP * L.CpR * sizeof(float) : (size_t)kPgWarps * 2 * L.CpR * sizeof(float);
+  if (bwd) o += (size_t)kPgWarps * kMaxKP * L.CpR * sizeof(float);
   L.total = align_up(o, 16);
   return L;
 }
@@ -241,7 +240,7 @@ __device__ __forceinline__ void pg_load_params(const AggArgs& a, const PgSmem& L
 
 // =================================================================================================
 //   BWD = false: centre = query q of cloud b, neighbour rows = feat_pm[idx[q][k]], k < ncount[q];
-//                out[b,:,q] = acc ; per-tile BatchNorm partial sums.                         (one tile per CTA)
+//                out[b,:,q] = acc ; per-tile BatchNorm partial moments.                      (one tile per CTA)
 //   BWD = true : centre = support point j, neighbour rows = g_pm[q_e] over the transposed list of j;
 //                out[b,:,j] = acc ; d/dWk accumulated per warp in shared memory.            (persistent tiles)
 // =================================================================================================
@@ -286,7 +285,6 @@ __global__ void __launch_bounds__(kPgWarps * 32, BWD ? 3 : 4) pg2_kernel(const A
     const float* rows = (BWD ? a.g_pm : a.feat_pm) + (size_t)b * R * a.Cp + c0 + cl;
     const float* cxyz = (BWD ? a.support_xyz : a.query_xyz) + (size_t)b * P * 3;   // centres
     const float* nxyz = (BWD ? a.query_xyz : a.support_xyz) + (size_t)b * R * 3;   // neighbours
-    float4 bn1 = make_float4(0.f, 0.f, 0.f, 0.f), bn2 = bn1;                        // forward: sum, sum of squares
 
     for (int pl = warp; pl < kPgTile; pl += kPgWarps) {
       const int p = p0 + pl;
@@ -340,22 +338,11 @@ __global__ void __launch_bounds__(kPgWarps * 32, BWD ? 3 : 4) pg2_kernel(const A
           __syncwarp();
         }
       }
-      if constexpr (!BWD) {
-        bn1.x += acc.x, bn1.y += acc.y, bn1.z += acc.z, bn1.w += acc.w;
-        ffma2(acc.x, acc.y, acc.x, acc.y, bn2.x, bn2.y);
-        ffma2(acc.z, acc.w, acc.z, acc.w, bn2.z, bn2.w);
-      }
       if (owner) {
         s_out[(size_t)(cl + 0) * (kPgTile + 1) + pl] = acc.x;
         s_out[(size_t)(cl + 1) * (kPgTile + 1) + pl] = acc.y;
         s_out[(size_t)(cl + 2) * (kPgTile + 1) + pl] = acc.z;
         s_out[(size_t)(cl + 3) * (kPgTile + 1) + pl] = acc.w;
-      }
-    }
-    if constexpr (!BWD) {
-      if (owner && a.partial) {  // this warp's sums over its centre points of the tile
-        *reinterpret_cast<float4*>(s_aux + ((size_t)warp * 2 + 0) * L.CpR + cl) = bn1;
-        *reinterpret_cast<float4*>(s_aux + ((size_t)warp * 2 + 1) * L.CpR + cl) = bn2;
       }
     }
     __syncthreads();
@@ -364,15 +351,9 @@ __global__ void __launch_bounds__(kPgWarps * 32, BWD ? 3 : 4) pg2_kernel(const A
     for (int c = warp; c < Cv; c += kPgWarps)
       if (p < P) store_out<TO>(s_out[(size_t)c * (kPgTile + 1) + lane], a, ((size_t)b * a.C + c0 + c) * P + p);
     if constexpr (!BWD) {
-      if (a.partial) {  // BatchNorm partial sums of the tile: the warps' sums in a fixed order
-        for (int e = threadIdx.x; e < 2 * Cv; e += blockDim.x) {
-          const int s2 = e / Cv, c = e % Cv;
-          float t = 0.f;
-#pragma unroll
-          for (int w = 0; w < kPgWarps; ++w) t += s_aux[((size_t)w * 2 + s2) * L.CpR + c];
-          a.partial[((size_t)tile * 2 + s2) * a.C + c0 + c] = t;
-        }
-      }
+      if (a.partial)  // BatchNorm partial moments of the tile, from the output tile in query order
+        for (int c = threadIdx.x; c < Cv; c += blockDim.x)
+          row_bn_moments(a.partial, tile, a.C, c0 + c, s_out + (size_t)c * (kPgTile + 1), min(kPgTile, P - p0));
     }
     __syncthreads();
   }
@@ -616,8 +597,8 @@ __device__ __forceinline__ int pg3_sum_index(int lane, int j) {
   return r2 < H2 && r1 < H1 && r0 < V ? r0 : -1;  // else a padding slot
 }
 
-// BWD = false: centre = query q of cloud b, rows = feat_pm[idx[q][k]], k < ncount[q]; out[b,:,q] = agg and one
-//              BatchNorm partial row (sum, sum of squares over the tile's 32 queries) per tile.
+// BWD = false: centre = query q of cloud b, rows = feat_pm[idx[q][k]], k < ncount[q]; out[b,:,q] = agg and per tile
+//              the BatchNorm partial moments (store_bn_moments).
 // BWD = true : centre = support point j, rows = g_pm[q_e] over the transposed list of j; out[b,:,j] = d/df and
 //              d/dWk in registers -> one partial row per CTA.
 template <bool BWD, int NT, typename TO>
@@ -770,16 +751,9 @@ __device__ __forceinline__ void pg3_body(const AggArgs& a, int partial_rows) {
         else store_out<TO>(s_out[(size_t)c * (kPgTile + 1) + lane], a, ((size_t)b * a.C + c0 + c) * P + p);
       }
     if constexpr (!BWD) {
-      if (a.partial) {  // BatchNorm partial sums of the tile, over its 32 queries in order (absent ones hold 0)
-        for (int e = threadIdx.x; e < 2 * Cv; e += blockDim.x) {
-          const int s2 = e / Cv, c = e % Cv;
-          const float* o = s_out + (size_t)c * (kPgTile + 1);
-          float sum = 0.f;
-#pragma unroll
-          for (int q = 0; q < kPgTile; ++q) sum = s2 ? fmaf(o[q], o[q], sum) : sum + o[q];
-          a.partial[((size_t)tile * 2 + s2) * a.C + c0 + c] = sum;
-        }
-      }
+      if (a.partial)  // BatchNorm partial moments of the tile, over its present queries in order
+        for (int c = threadIdx.x; c < Cv; c += blockDim.x)
+          row_bn_moments(a.partial, tile, a.C, c0 + c, s_out + (size_t)c * (kPgTile + 1), min(kPgTile, P - p0));
     }
     __syncthreads();
   }

@@ -11,7 +11,8 @@
 // The per-point terms are ONE (B*N x (C+3)) x ((C+3) x 2*Cop) product over the augmented point-major matrix
 // [f | s/r] (csrc/gemm.cu); the per-neighbour work that remains is a row gather with 6 instructions per
 // element.  BatchNorm2d statistics over all B*M*K positions (padding slots included, as in the reference) are
-// accumulated on the fly:  sum_k y = K a' + S,  sum_k y^2 = K a'^2 + 2 a' S + S2  with S = sum_k bv.
+// accumulated on the fly as centred moments (store_bn_moments): per query about its slot-0 value y_0 = a' + bv[j_0],
+// sum_k (y - y_0) = sum_k (bv[j_k] - bv[j_0]) and likewise the squares, merged per warp and per tile.
 // The max over K commutes with the monotone BN + ReLU; which extremum is needed depends only on the sign of
 // gamma, so the host folds sgn = sign(gamma) into the T rows of the product (t = sgn*bv) and the kernel tracks
 // max_k t with its FIRST arg-max slot (max_pool2d's tie rule):  y_sel = a' + sgn*max_k t,
@@ -45,7 +46,7 @@ struct PwArgs {
   float* aq;                 // (B,M,Cop) a'
   float* sq;                 // (B,M,Cop) S = sum_k bv
   unsigned char* karg;       // (B,M,Cop) first arg-max slot
-  float* partial;            // fwd: (ntiles,2,Cout) ; bwd sparse: (ntiles,3,Cout) dWp partials
+  float* partial;            // fwd: (ntiles,kBnRows,Cout) ; bwd sparse: (ntiles,3,Cout) dWp partials
   // backward only
   const float* grad_out;     // unused, kept for the layout of this block: pwmlp_bwd_stats_kernel takes grad_out as
   const float* out;          // a kernel argument, and nothing reads out
@@ -72,14 +73,18 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_fwd_kernel(const PwArgs a
   const int chunkC = min(32 * CI, a.Cop - c0);
   int* s_idx = reinterpret_cast<int*>(smem) + (size_t)warp * a.K;                       // [warps][K]
   float* s_y = reinterpret_cast<float*>(smem + align_up((size_t)kPWWarps * a.K * 4, 16));  // [chunk][tile+1]
-  float* s_red = s_y + (size_t)32 * CI * (kPWTile + 1);                                  // [warps][2][chunk]
+  float* s_red = s_y + (size_t)32 * CI * (kPWTile + 1);                                  // [warps][4][chunk]
 
   const int tiles_per_cloud = (a.M + kPWTile - 1) / kPWTile;
   const int b = blockIdx.x / tiles_per_cloud;
   const int q0 = (blockIdx.x % tiles_per_cloud) * kPWTile;
 
   bool okc[CI];
-  float wpx[CI], wpy[CI], wpz[CI], sg[CI], s1[CI], s2[CI];
+  // BatchNorm moments of this warp's y values about its first query's slot-0 value z = aw + sg * tw (exact; aw, tw
+  // kept in s_red): sum (y - z) and sum (y - z)^2, accumulated from each query's own moments about its slot-0 value
+  float wpx[CI], wpy[CI], wpz[CI], sg[CI], dw[CI], qw[CI];
+  float* s_aw = s_red + (size_t)warp * 4 * 32 * CI + lane;  // [0][chunk] aw, [1][chunk] tw: this lane's own words
+  float* s_tw = s_aw + 32 * CI;
 #pragma unroll
   for (int i = 0; i < CI; ++i) {
     okc[i] = lane + 32 * i < chunkC;
@@ -89,7 +94,8 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_fwd_kernel(const PwArgs a
     wpy[i] = ok ? a.wp[c * 3 + 1] : 0.f;
     wpz[i] = ok ? a.wp[c * 3 + 2] : 0.f;
     sg[i] = ok ? a.sgn[c] : 1.f;
-    s1[i] = s2[i] = 0.f;
+    dw[i] = qw[i] = 0.f;
+    s_aw[32 * i] = s_tw[32 * i] = 0.f;
   }
   const float* ab = a.ab_pm + (size_t)b * a.N * 2 * a.Cop + c0 + lane;  // per-lane base pointer (A half)
   const float* tb = ab + a.Cop;                                           // T half
@@ -128,14 +134,17 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_fwd_kernel(const PwArgs a
                   qy = __fmul_rn(__fsub_rn(a.query_xyz[gq * 3 + 1], org[1]), a.inv_radius),
                   qz = __fmul_rn(__fsub_rn(a.query_xyz[gq * 3 + 2], org[2]), a.inv_radius);
       __syncwarp();
-      float ap[CI], S[CI], S2[CI], m[CI];
+      // S = sum_k t; D, Q = sum_k (t - t0), sum_k (t - t0)^2 about the slot-0 value t0
+      float ap[CI], S[CI], t0[CI], D[CI], Q[CI], m[CI];
       int km[CI];
       {
         const float* arow = row_at(ab, (unsigned)s_idx[0]);
+        const float* trow = row_at(tb, (unsigned)s_idx[0]);
 #pragma unroll
         for (int i = 0; i < CI; ++i) {
           ap[i] = __ldg(arow + 32 * i) - fmaf(wpz[i], qz, fmaf(wpy[i], qy, wpx[i] * qx));
-          S[i] = S2[i] = 0.f;
+          t0[i] = __ldg(trow + 32 * i);
+          S[i] = D[i] = Q[i] = 0.f;
           m[i] = -INFINITY;
           km[i] = 0;
         }
@@ -153,9 +162,10 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_fwd_kernel(const PwArgs a
         for (int u = 0; u < kPWU; ++u)
 #pragma unroll
           for (int i = 0; i < CI; ++i) {
-            const float t = v[u][i];
+            const float t = v[u][i], e = t - t0[i];
             S[i] += t;
-            S2[i] = fmaf(t, t, S2[i]);
+            D[i] += e;
+            Q[i] = fmaf(e, e, Q[i]);
             const bool gt = t > m[i];  // strict: the first occurrence keeps the slot, as max_pool2d
             m[i] = gt ? t : m[i];
             km[i] = gt ? (k0 + u) : km[i];
@@ -165,9 +175,10 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_fwd_kernel(const PwArgs a
         const float* row = row_at(tb, (unsigned)s_idx[k0]);
 #pragma unroll
         for (int i = 0; i < CI; ++i) {
-          const float t = __ldg(row + 32 * i);
+          const float t = __ldg(row + 32 * i), e = t - t0[i];
           S[i] += t;
-          S2[i] = fmaf(t, t, S2[i]);
+          D[i] += e;
+          Q[i] = fmaf(e, e, Q[i]);
           const bool gt = t > m[i];
           m[i] = gt ? t : m[i];
           km[i] = gt ? k0 : km[i];
@@ -178,8 +189,11 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_fwd_kernel(const PwArgs a
       for (int i = 0; i < CI; ++i) {
         const float Sb = sg[i] * S[i];             // sum_k bv
         ys[i] = ap[i] + sg[i] * m[i];              // selected extremum of y
-        s1[i] += fmaf(fK, ap[i], Sb);              // sum_k y
-        s2[i] += fmaf(fK * ap[i], ap[i], fmaf(2.f * ap[i], Sb, S2[i]));  // sum_k y^2
+        if (ql == warp) s_aw[32 * i] = ap[i], s_tw[32 * i] = t0[i];
+        // y_k - z = e + sg (t_k - t0), e = this query's slot-0 value about z
+        const float e = (ap[i] - s_aw[32 * i]) + sg[i] * (t0[i] - s_tw[32 * i]), dq = sg[i] * D[i];
+        dw[i] += fmaf(fK, e, dq);
+        qw[i] += fmaf(fK * e, e, fmaf(2.f * e, dq, Q[i]));
         if (lane + 32 * i < chunkC) {
           const size_t o = gq * a.Cop + c0 + lane + 32 * i;
           a.aq[o] = ap[i];
@@ -193,8 +207,8 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_fwd_kernel(const PwArgs a
   }
 #pragma unroll
   for (int i = 0; i < CI; ++i) {
-    s_red[((size_t)warp * 2 + 0) * 32 * CI + lane + 32 * i] = s1[i];
-    s_red[((size_t)warp * 2 + 1) * 32 * CI + lane + 32 * i] = s2[i];
+    s_red[((size_t)warp * 4 + 2) * 32 * CI + lane + 32 * i] = dw[i];
+    s_red[((size_t)warp * 4 + 3) * 32 * CI + lane + 32 * i] = qw[i];
   }
   __syncthreads();
   const int q = q0 + lane;
@@ -206,14 +220,20 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_fwd_kernel(const PwArgs a
   for (int cl = threadIdx.x; cl < 32 * CI; cl += blockDim.x) {
     const int c = c0 + cl;
     if (c >= a.Cout) continue;
-    float t1 = 0.f, t2 = 0.f;
-#pragma unroll
-    for (int w = 0; w < kPWWarps; ++w) {
-      t1 += s_red[((size_t)w * 2 + 0) * 32 * CI + cl];
-      t2 += s_red[((size_t)w * 2 + 1) * 32 * CI + cl];
+    // the tile's centre: warp 0's z rounded to fp32, r = z - ctr exactly (two-sum)
+    const float sgc = a.sgn[c], a0 = s_red[cl], t0 = sgc * s_red[32 * CI + cl];
+    const float ctr = a0 + t0, bb = ctr - a0, r = (a0 - (ctr - bb)) + (t0 - bb);
+    const int nq = min(kPWTile, a.M - q0);
+    float d = 0.f, q2 = 0.f;
+    for (int w = 0; w < kPWWarps && w < nq; ++w) {  // warps in a fixed order, each about z_w = ctr + g
+      const float* sw = s_red + (size_t)w * 4 * 32 * CI + cl;
+      const float nw = fK * (float)((nq - w + kPWWarps - 1) / kPWWarps);
+      const float g = (sw[0] - a0) + sgc * (sw[32 * CI] - s_red[32 * CI + cl]) + r;
+      const float dwv = sw[2 * 32 * CI], qwv = sw[3 * 32 * CI];
+      q2 += fmaf(nw * g, g, fmaf(2.f * g, dwv, qwv));
+      d += fmaf(nw, g, dwv);
     }
-    a.partial[((size_t)blockIdx.x * 2 + 0) * a.Cout + c] = t1;
-    a.partial[((size_t)blockIdx.x * 2 + 1) * a.Cout + c] = t2;
+    store_bn_moments(a.partial, blockIdx.x, a.Cout, c, fK * (float)nq, ctr, d, q2);
   }
 }
 
@@ -279,22 +299,21 @@ __global__ void __launch_bounds__(256) pwmlp_bwd_stats_kernel(const TG* __restri
 }
 
 // Support-major pass over the all-slots CSR lists of point j (no float atomics): dense part of d/dbv
-//   grad_T[j] = sgn * ( -cnt*c1 - c2*(sum_e a'[q_e] + cnt*(bv[j] - mean)) ),   grad_A[j] = 0
+//   grad_T[j] = sgn * ( -cnt*c1 - c2*(sum_e (a'[q_e] - a0) + cnt*(bv[j] + a0 - mean)) ),   grad_A[j] = 0
+// a0 = a' of the cloud's first query: the sum then adds spread-sized terms, where sum_e a'[q_e] and cnt*(bv - mean)
+// would cancel to (y - mean) only after cnt fp32 additions of |a'|-sized ones (a channel whose mean dwarfs its spread)
 template <int CI>
 __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_bwd_dense_kernel(const PwArgs a) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c0 = blockIdx.y * 32 * CI;
   const int chunkC = min(32 * CI, a.Cop - c0);
-  bool okc[CI];
-  float c1[CI], c2[CI], mean[CI], sg[CI];
+  float c1[CI], c2[CI], sg[CI];  // the mean is read where it is used: a0 below takes its register
 #pragma unroll
   for (int i = 0; i < CI; ++i) {
-    okc[i] = lane + 32 * i < chunkC;
     const int c = c0 + lane + 32 * i;
     const bool ok = c < a.Cout;
     const float invstd = ok ? a.stats[a.Cout + c] : 0.f;
     const float sc = ok ? invstd * a.gamma[c] : 0.f;
-    mean[i] = ok ? a.stats[c] : 0.f;
     c1[i] = ok ? sc * a.dgb[a.Cout + c] * a.inv_count : 0.f;
     c2[i] = ok ? sc * invstd * a.dgb[c] * a.inv_count : 0.f;
     sg[i] = ok ? a.sgn[c] : 1.f;
@@ -304,6 +323,9 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_bwd_dense_kernel(const Pw
     const int b = tile / per_cloud;
     const int j0 = (tile % per_cloud) * kPWTile;
     const float* aq = a.aq + (size_t)b * a.M * a.Cop + c0 + lane;  // per-lane base pointer
+    float a0[CI];
+#pragma unroll
+    for (int i = 0; i < CI; ++i) a0[i] = __ldg(aq + 32 * i);
     const int* off = a.csr_off + (size_t)b * (a.N + 1);
     const int* ent = a.csr_ent + (size_t)b * a.M * a.K;
     for (int jl = warp; jl < kPWTile; jl += kPWWarps) {
@@ -328,12 +350,12 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_bwd_dense_kernel(const Pw
 #pragma unroll
           for (int u = 0; u < kPWU; ++u)
 #pragma unroll
-            for (int i = 0; i < CI; ++i) acc[i] += v[u][i];
+            for (int i = 0; i < CI; ++i) acc[i] += v[u][i] - a0[i];
         }
         for (; r < rows; ++r) {
           const float* row = row_at(aq, __shfl_sync(0xffffffffu, myq, r));
 #pragma unroll
-          for (int i = 0; i < CI; ++i) acc[i] += __ldg(row + 32 * i);
+          for (int i = 0; i < CI; ++i) acc[i] += __ldg(row + 32 * i) - a0[i];
         }
       }
       const float cnt = (float)(e1 - e0);
@@ -341,12 +363,13 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_bwd_dense_kernel(const Pw
       float* grow = a.grad_ab_pm + ((size_t)b * a.N + j) * 2 * a.Cop;
 #pragma unroll
       for (int i = 0; i < CI; ++i) {
-        if (okc[i]) {
+        const int c = c0 + lane + 32 * i;
+        if (lane + 32 * i < chunkC && c < a.Cout) {
           const float bv = sg[i] * __ldg(trow + 32 * i);
-          const float dbv = -cnt * c1[i] - c2[i] * (acc[i] + cnt * (bv - mean[i]));
+          const float dbv = -cnt * c1[i] - c2[i] * (acc[i] + cnt * ((bv + a0[i]) - __ldg(a.stats + c)));
           // grad_ab is zero-filled by the entry point; the query pass adds its arg-max hits to the same words
           // concurrently, so this is a reduction too (one per word: no contention)
-          if (c0 + lane + 32 * i < a.Cout) atomicAdd(&grow[a.Cop + c0 + lane + 32 * i], sg[i] * dbv);
+          atomicAdd(&grow[a.Cop + c], sg[i] * dbv);
         }
       }
     }
@@ -511,7 +534,7 @@ static int pw_ci(int Cop) {
 template <int CI>
 static int launch_pw_fwd(const PwArgs& a, cudaStream_t stream) {
   const size_t smem = align_up((size_t)kPWWarps * a.K * 4, 16) + (size_t)32 * CI * (kPWTile + 1) * 4 +
-                      (size_t)kPWWarps * 2 * 32 * CI * 4;
+                      (size_t)kPWWarps * 4 * 32 * CI * 4;
   static std::atomic<unsigned long long> seen{0};
   allow_big_smem(pwmlp_fwd_kernel<CI>, seen);
   dim3 grid(a.ntiles, ceil_div(a.Cop, 32 * CI));

@@ -51,7 +51,7 @@ class _FusedAggBNReLU(Function):
             L = ops._lib.lib()
             agg = torch.empty(B, C, M, dtype=torch.float32, device=features.device)
             tpc = L.cl3d_agg_num_tiles(1, M)      # BatchNorm partial rows per cloud
-            partial = torch.empty(B * tpc, 2, C, dtype=torch.float32, device=features.device) if training else None
+            partial = ops.bn_partial_buffer(B * tpc, C, features.device) if training else None
             cur = torch.cuda.current_stream()
             for b0, b1, ev in nl.parts:
                 cur.wait_event(ev)

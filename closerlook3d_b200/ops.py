@@ -213,12 +213,26 @@ def reduce_partials(partial):
 # --------------------------------------------------------------------------------------------------
 FAM_POSPOOL_XYZ, FAM_POSPOOL_SINCOS, FAM_ADAPTIVE_DP, FAM_PSEUDOGRID = 0, 1, 2, 3
 REDUCE = {"avg": 0, "mean": 0, "sum": 1, "max": 2}
+BN_PARTIAL_ROWS = 4  # CL3D_BN_PARTIAL_ROWS: per tile and channel n, centre c, sum (x - c), sum (x - c)^2
+
+
+def bn_partial_buffer(ntiles, C, device):
+    """(ntiles, BN_PARTIAL_ROWS, C) fp32: a forward's per-tile BatchNorm moments, rows of one tile contiguous"""
+    return torch.empty(ntiles, BN_PARTIAL_ROWS, C, dtype=F32, device=device)
+
+
+def bn_partial_moments(partial):
+    """(ntiles, BN_PARTIAL_ROWS, C) -> float64 (n, sum, M2) per tile and channel, each (ntiles, C); M2 = the tile's
+    sum of squared deviations from its own mean"""
+    p = partial.double()
+    n, c, d, q = p[:, 0], p[:, 1], p[:, 2], p[:, 3]
+    return n, n * c + d, q - d * d / n
 
 
 @_on_device
 def agg_fwd(family, reduction, feat_pm, query_xyz, support_xyz, idx, ncount, p0, p1, C, radius, normalize, shared=1,
             nkp=0, extent=1.0, influence=0, want_bn_partial=True, out=None, arg=None):
-    """-> (agg (B,C,M), bn_partial (ntiles,2,C) | None); out = (agg, partial) preallocated (e.g. batch slices);
+    """-> (agg (B,C,M), bn_partial (ntiles,BN_PARTIAL_ROWS,C) | None); out = (agg, partial) preallocated (e.g. batch slices);
     arg = (B,M,Cp) uint8 buffer for the winning slots, required by (and only by) the max reduction"""
     B, N, Cp = feat_pm.shape
     M, K = idx.shape[1], idx.shape[2]
@@ -228,7 +242,7 @@ def agg_fwd(family, reduction, feat_pm, query_xyz, support_xyz, idx, ncount, p0,
         agg, partial = out
     else:
         agg = torch.empty(B, C, M, dtype=F32, device=dev)
-        partial = torch.empty(L.cl3d_agg_num_tiles(B, M), 2, C, dtype=F32, device=dev) if want_bn_partial else None
+        partial = bn_partial_buffer(L.cl3d_agg_num_tiles(B, M), C, dev) if want_bn_partial else None
     check(L.cl3d_agg_fwd(family, reduction, ptr(feat_pm), ptr(query_xyz), ptr(support_xyz), ptr(idx), ptr(ncount),
                          ptr(p0), ptr(p1), B, N, M, K, C, float(radius), int(normalize), int(shared), int(nkp),
                          float(extent), int(influence), ptr(agg), ptr(partial), ptr(arg), stream_ptr()), "cl3d_agg_fwd")
@@ -358,7 +372,7 @@ def pwmlp_fwd_stats(ab_pm, wp, sgn, query_xyz, support_xyz, idx, Cout, radius):
     aq = _empty_pm(B, M, Cop, dev)
     sq = torch.empty(B, M, Cop, dtype=F32, device=dev)
     karg = torch.empty(B, M, Cop, dtype=torch.uint8, device=dev)
-    partial = torch.empty(L.cl3d_agg_num_tiles(B, M), 2, Cout, dtype=F32, device=dev)
+    partial = bn_partial_buffer(L.cl3d_agg_num_tiles(B, M), Cout, dev)
     check(L.cl3d_pwmlp_fwd_stats(ptr(ab_pm), ptr(wp), ptr(sgn), ptr(query_xyz), ptr(support_xyz), ptr(idx), B, N, M, K, Cout,
                                  float(radius), ptr(ysel), ptr(aq), ptr(sq), ptr(karg), ptr(partial), stream_ptr()),
           "cl3d_pwmlp_fwd_stats")

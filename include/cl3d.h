@@ -178,8 +178,8 @@ int cl3d_to_channel_major(const float* in_nc, int B, int C, int N, void* out_cn,
  *                                `influence` 0 = linear, 1 = constant
  *   normalize : 1 -> dp /= radius (pt_utils.py:128-129; PosPool/AdaptiveWeight), 0 -> raw (PseudoGrid)
  *   agg       (B,C,M) channel-major out (pre-BN)
- *   bn_partial (ntiles, 2, C) out: per-tile sum and sum of squares of agg (for the out_transform BN);
- *               ntiles = cl3d_agg_num_tiles(B,M).  May be NULL.
+ *   bn_partial (ntiles, CL3D_BN_PARTIAL_ROWS, C) out: per-tile moments of agg for the out_transform BN (see
+ *               cl3d_bn_finalize); ntiles = cl3d_agg_num_tiles(B,M), the tiles of one cloud contiguous.  May be NULL.
  * backward (gather form over the CSR lists; no float atomics on activations):
  *   g_pm      (B,M,Cp) point-major d(loss)/d(agg)
  *   grad_feat (B,C,N) channel-major out in `dtype`, fully written (by each backward kernel's own channel-major store)
@@ -212,13 +212,17 @@ int cl3d_reduce_partials(const float* partial, int ntiles, int P, float* out, cl
 /* ------------------------------------------------------------------------------------------------
  * out_transform = BatchNorm1d + ReLU (local_aggregation_operators.py:43-45,110), channel-major (B,C,M).
  *   bn_finalize: from the per-tile partials -> batch mean / invstd (save_stats (2,C)), updates running
- *                stats with `momentum` (unbiased variance, as nn.BatchNorm1d) when training.
+ *                stats with `momentum` (unbiased variance, as nn.BatchNorm1d) when training.  A forward's
+ *                partials hold, per tile and channel, CL3D_BN_PARTIAL_ROWS rows: n (number of values), c (a
+ *                centre near the tile's values), sum (x - c), sum (x - c)^2.  The tiles are merged in
+ *                double, so a channel whose mean dwarfs its spread keeps its variance.
  *   bn_relu_fwd: y = relu((x-mean)*invstd*gamma + beta); in eval mode pass stats made from running stats.
  *   bn_relu_bwd_stats / bn_relu_bwd_apply: two-phase backward; apply writes d(loss)/d(agg) POINT-MAJOR
  *                (B,M,Cp) ready for cl3d_agg_bwd, and dgamma/dbeta.
  *   y written / grad_y read in `dtype`; x, the statistics, partials, dgamma_dbeta and g_pm fp32.
  * ---------------------------------------------------------------------------------------------- */
-int cl3d_bn_finalize(const float* bn_partial, int ntiles, int C, long long count, float eps,
+#define CL3D_BN_PARTIAL_ROWS 4
+int cl3d_bn_finalize(const float* bn_partial /*(ntiles,CL3D_BN_PARTIAL_ROWS,C)*/, int ntiles, int C, long long count, float eps,
                      float momentum, int training, float* running_mean, float* running_var,
                      float* save_stats /*(2,C): mean, invstd*/, cl3d_stream_t stream);
 int cl3d_bn_relu_fwd(const float* x, const float* save_stats, const float* gamma, const float* beta,
@@ -255,7 +259,7 @@ int cl3d_sgemm_algo(const float* a, long long sa_m, long long sa_k, const float*
  *   ab_pm (B,N,2*Cop)       : row = [A | T],  A = (Wc-Wr) f,  T = sgn*(Wr f + Wp s/r)   (one cl3d_sgemm_algo)
  *   wp (Cout,3), sgn (Cout) : conv weight columns 0..2; sign(gamma) as +-1.0
  * fwd_stats : ysel (B,Cout,M) selected extremum of y; aq, sq (B,M,Cop) a' and sum_k bv; karg (B,M,Cop) uint8
- *             first arg-max slot (K <= 255); bn_partial (cl3d_agg_num_tiles(B,M), 2, Cout) -> cl3d_bn_finalize
+ *             first arg-max slot (K <= 255); bn_partial (cl3d_agg_num_tiles(B,M), CL3D_BN_PARTIAL_ROWS, Cout) -> cl3d_bn_finalize
  *             with count = B*M*K.
  * fwd_out   : out (B,Cout,M) = relu(sc*ysel + sh), in `dtype`.
  * bwd       : grad_out (B,Cout,M) in `dtype`.  The ReLU decision is recomputed from ysel, save_stats, gamma and beta

@@ -225,6 +225,8 @@ def pointwise_mlp(ext, st, cfg, cin, cout, radius, nsample, q_xyz, s_xyz, q_mask
     x = torch.cat([dp, center, gf - center], 1)
     for i in range(pw.num_mlps):                                              # :252-272 conv + BN2d + ReLU
         x = F.conv2d(x, st[f"mlps.conv{i}.0.weight"])
+        if KEEP is not None:
+            KEEP[f"pwmlp_prebn{i}"] = x.detach()                              # what BatchNorm2d normalises
         y = _bn(x, st, f"mlps.conv{i}.1", cfg.bn_momentum, training)
         x = F.relu(y)
     if KEEP is not None:

@@ -50,5 +50,9 @@ def test_pg_v2_matches_v1(cuda, B, N, K, C, influence):
     for x1, x2, what in ((g1, g2, "d/df"), (w1, w2, "d/dWk"), (a1, a2, "forward")):
         err = float((x1 - x2).abs().max()) / max(1.0, float(x1.abs().max()))
         assert err <= 5e-6, f"{what}: v2 differs from v1 by {err:.2e}"
-    s1, s2 = p1.sum(0), p2.sum(0)   # BatchNorm partial sums (tile sizes are the same: 32 queries)
-    assert float((s1 - s2).abs().max()) <= 1e-5 * max(1.0, float(s1.abs().max()))
+    # BatchNorm partial moments (tile sizes are the same: 32 queries): counts, and the sums and sums of squared
+    # deviations over the tiles
+    (n1, s1, q1), (n2, s2, q2) = ops.bn_partial_moments(p1), ops.bn_partial_moments(p2)
+    assert torch.equal(n1, n2)
+    for x1, x2 in ((s1.sum(0), s2.sum(0)), (q1.sum(0), q2.sum(0))):
+        assert float((x1 - x2).abs().max()) <= 1e-5 * max(1.0, float(x1.abs().max()))

@@ -1,8 +1,8 @@
 """Third-generation PseudoGrid forward (csrc/pg.cu pg3_fwd_kernel: per-kernel-point sums U = h^T f on the tensor cores
 with 3xTF32, then out = sum_k' Wk * U) against the second-generation kernel (CL3D_PG_V2=1) on the same inputs and
 lists, and both against a float64 evaluation of the same sums.  Same terms and the same influences; the sums are
-regrouped, so the comparison is to rounding, not bit for bit.  The BatchNorm partial rows keep their meaning: the sum
-and the sum of squares of the output over each tile of 32 queries.  The forward takes the third generation up to 40
+regrouped, so the comparison is to rounding, not bit for bit.  The BatchNorm partials keep their meaning: the moments
+(count, sum, sum of squared deviations from the tile mean) of the output over each tile of 32 queries.  The forward takes the third generation up to 40
 padded channels (C = 8, 36 below); the wider cases check that the dispatch still computes the same sums."""
 import pytest
 import torch
@@ -37,18 +37,33 @@ def _f64(c, influence):
     return torch.einsum("bmkp,pc,bcmk->bcm", h, c["wk"].double(), fj)
 
 
-def _tile_sums(agg):
-    """(ntiles, 2, C) float64: sum and sum of squares of agg over each tile of 32 queries of each cloud"""
+def _tile_moments(agg):
+    """(ntiles, 3, C) float64: count, sum and sum of squared deviations from the tile mean of agg over each tile of 32
+    queries of each cloud"""
     B, C, M = agg.shape
     T = (M + 31) // 32
+    present = (torch.arange(T * 32, device=agg.device) < M).view(T, 32)
     x = torch.zeros(B, C, T * 32, dtype=torch.float64, device=agg.device)
     x[..., :M] = agg.double()
     x = x.view(B, C, T, 32)
-    return torch.stack([x.sum(-1), (x * x).sum(-1)], -1).permute(0, 2, 3, 1).reshape(B * T, 2, C)   # row b * T + t
+    n = present.sum(-1).double().expand(B, C, T)
+    s = x.sum(-1)
+    m2 = torch.where(present, (x - (s / n)[..., None]) ** 2, 0.0).sum(-1)
+    return torch.stack([n, s, m2], -1).permute(0, 2, 3, 1).reshape(B * T, 3, C)   # row b * T + t
+
+
+def _moments(part):
+    return torch.stack(ops.bn_partial_moments(part), 1)
+
+
+def _stats(part, C, count):
+    rm, rv = torch.zeros(C, device=part.device), torch.ones(C, device=part.device)
+    st = ops.bn_finalize(part, C, count, 1e-5, 1.0, True, rm, rv)
+    return torch.stack([st[0], rv])   # mean, unbiased variance
 
 
 @pytest.mark.parametrize("B,N,K,C,nkp,influence,thin", CASES)
-@pytest.mark.parametrize("max_grid", [0, 5])
+@pytest.mark.parametrize("max_grid", [0, 1, 2, 5])   # 1 or 2 CTAs: each walks every tile of its share
 def test_pg_v3_fwd_matches_v2_and_f64(cuda, B, N, K, C, nkp, influence, thin, max_grid):
     c = _case(cuda, B, N, K, C, nkp, 91 + N + C, thin)
     if K > 32:
@@ -62,15 +77,24 @@ def test_pg_v3_fwd_matches_v2_and_f64(cuda, B, N, K, C, nkp, influence, thin, ma
     assert torch.equal(a3, a3b) and torch.equal(p3, p3b), "two runs of the same grid differ"
     assert _err(a3, a2) <= 1e-5, f"agg: v3 differs from v2 by {_err(a3, a2):.2e}"
     assert p3.shape == p2.shape
-    assert _err(p3, p2) <= 1e-5, f"BatchNorm partials: v3 differs from v2 by {_err(p3, p2):.2e}"
+    m2, m3 = _moments(p2), _moments(p3)
+    assert torch.equal(m3[:, 0], m2[:, 0]), "tile counts differ"
+    assert _err(m3, m2) <= 1e-5, f"BatchNorm partials: v3 differs from v2 by {_err(m3, m2):.2e}"
     ref = _f64(c, influence)
     e2, e3 = _err(a2, ref), _err(a3, ref)
-    ep = _err(p3, _tile_sums(ref))
+    mref = _tile_moments(ref)
+    assert torch.equal(m3[:, 0], mref[:, 0])
+    # per tile sum and sum of squares against float64 (the aggregation's error included), and the centred second
+    # moment against that of the kernel's own output
+    def sums(m):   # (ntiles, 2, C): sum and sum of squares
+        return torch.stack([m[:, 1], m[:, 2] + m[:, 1] ** 2 / m[:, 0]], 1)
+
+    ep = max(_err(sums(m3), sums(mref)), _err(m3[:, 2], _tile_moments(a3)[:, 2]))
     print(f"float64 reference: agg v2 {e2:.2e} v3 {e3:.2e} | v3 BatchNorm partials {ep:.2e}")
     assert e3 <= max(3 * e2, 2e-6), f"v3 {e3:.2e} against v2 {e2:.2e}"
     assert ep <= 1e-5
-    # BatchNorm statistics from the partial rows, as cl3d_bn_finalize sums them
-    s2, s3 = p2.double().sum(0), p3.double().sum(0)
+    # BatchNorm statistics from the partials, as cl3d_bn_finalize merges them
+    s2, s3 = _stats(p2, C, B * N), _stats(p3, C, B * N)
     assert float((s3 - s2).abs().max()) <= 1e-5 * max(1.0, float(s2.abs().max()))
 
 
