@@ -25,18 +25,18 @@ SIGNATURES = {
     "cl3d_launch_count": (_ll, []),
     "cl3d_ball_query_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "cl3d_ball_query_algo": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _sz, _i, _vp]),
-    "cl3d_ball_query_csr_workspace_bytes": (_sz, [_i, _i, _i, _i]),
-    "cl3d_ball_query_csr": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _sz, _i, _i, _vp]),
+    "cl3d_ball_query_csr_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "cl3d_ball_query_csr": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _sz, _i, _i, _i, _vp]),
     "cl3d_nearest_query_workspace_bytes": (_sz, [_i, _i, _i]),
     "cl3d_nearest_query": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
-    "cl3d_csr_workspace_bytes": (_sz, [_i, _i, _i, _i]),
-    "cl3d_build_csr": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "cl3d_csr_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "cl3d_build_csr": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _i, _vp]),
     "cl3d_group_points": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
-    "cl3d_group_points_grad": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "cl3d_group_points_grad": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "cl3d_grid_subsample_workspace_bytes": (_sz, [_i, _i, _i]),
     "cl3d_grid_subsample": (_i, [_vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _sz, _vp]),
     "cl3d_gather_max_fwd": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp]),
-    "cl3d_gather_max_bwd": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "cl3d_gather_max_bwd": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "cl3d_to_point_major": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "cl3d_to_channel_major": (_i, [_vp, _i, _i, _i, _vp, _i, _vp]),
     "cl3d_agg_num_tiles": (_i, [_i, _i]),
@@ -57,8 +57,8 @@ SIGNATURES = {
     "cl3d_to_point_major_aug": (_i, [_vp, _i, _vp, _i, _i, _i, _f, _vp, _vp]),
     "cl3d_pwmlp_fwd_stats": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp]),
     "cl3d_pwmlp_fwd_out": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp]),
-    "cl3d_pwmlp_bwd_scratch_floats": (_sz, [_i, _i, _i, _i]),
-    "cl3d_pwmlp_bwd": (_i, [_vp, _i] + [_vp] * 15 + [_i, _i, _i, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "cl3d_pwmlp_bwd_scratch_floats": (_sz, [_i, _i, _i, _i, _i]),
+    "cl3d_pwmlp_bwd": (_i, [_vp, _i] + [_vp] * 15 + [_i, _i, _i, _i, _i, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "cl3d_mhead_save_floats": (_sz, [_i, _i]),
     "cl3d_mhead_fwd_workspace_bytes": (_sz, [_vp, _i, _i]),
     "cl3d_mhead_bwd_workspace_bytes": (_sz, [_vp, _i, _i]),

@@ -132,6 +132,24 @@ __global__ void __launch_bounds__(256) group_points_grad_kernel(const T* __restr
   atomicAdd(gp + idx[(size_t)b * M * K + e], load_f32(grad_out + ((size_t)b * C + c) * M * K + e));
 }
 
+// gather form over the transposed lists of idx (all K slots): grad_points[b,c,j] = sum of grad_out[b,c,e] over the
+// entries e = q*K + k of j's list, in list order, rounded once to T.  Canonical lists give the same bits every run.
+template <typename T>
+__global__ void __launch_bounds__(256) group_points_grad_csr_kernel(const T* __restrict__ grad_out,
+                                                                    const int* __restrict__ csr_off,
+                                                                    const int* __restrict__ csr_ent, int C, int N,
+                                                                    int M, int K, T* __restrict__ grad_points) {
+  const int b = blockIdx.z, c = blockIdx.y;
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  const int o0 = csr_off[(size_t)b * (N + 1) + j], o1 = csr_off[(size_t)b * (N + 1) + j + 1];
+  const int* ent = csr_ent + (size_t)b * M * K;
+  const T* g = grad_out + ((size_t)b * C + c) * M * K;
+  float acc = 0.f;
+  for (int p = o0; p < o1; ++p) acc += load_f32(g + ent[p]);
+  store_f32(grad_points + ((size_t)b * C + c) * N + j, acc);
+}
+
 // the 16-bit group_points gradient: fp32 accumulation buffer -> dtype, one rounding per element
 template <typename T>
 __global__ void __launch_bounds__(256) convert_kernel(const float* __restrict__ in, size_t n, T* __restrict__ out) {
@@ -173,7 +191,7 @@ __global__ void __launch_bounds__(1024) reduce_partials_kernel(const float* __re
 
 using namespace cl3d;
 
-extern "C" int cl3d_version(void) { return 102; }
+extern "C" int cl3d_version(void) { return 103; }
 extern "C" const char* cl3d_last_error(void) { return g_err; }
 extern "C" int cl3d_padded_channels(int C) { return padded_channels(C); }
 extern "C" int cl3d_sm_count(void) { return sm_count(); }
@@ -227,14 +245,27 @@ extern "C" int cl3d_group_points(const void* points, int dtype, const int* idx, 
 }
 
 extern "C" int cl3d_group_points_grad(const void* grad_out, int dtype, const int* idx, int B, int C, int N, int M,
-                                      int K, void* grad_points, float* acc, cl3d_stream_t stream_) {
+                                      int K, const int* csr_off, const int* csr_ent, void* grad_points, float* acc,
+                                      cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(B >= 0 && C >= 1 && N >= 1 && M >= 0 && K >= 1 && grad_out && idx && grad_points,
                "cl3d_group_points_grad: bad arguments");
   CL3D_REQUIRE(C <= 65535 && B <= 65535, "cl3d_group_points_grad: C or B too large");
+  CL3D_REQUIRE(!csr_off == !csr_ent, "cl3d_group_points_grad: csr_off and csr_ent are both given or both NULL");
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_group_points_grad");
-  CL3D_REQUIRE(dtype == CL3D_DTYPE_F32 || acc, "cl3d_group_points_grad: a 16-bit gradient needs the fp32 buffer acc");
+  CL3D_REQUIRE(dtype == CL3D_DTYPE_F32 || acc || csr_off,
+               "cl3d_group_points_grad: a 16-bit gradient needs the fp32 buffer acc");
   if (B == 0) return CL3D_OK;
+  if (csr_off) {
+    return with_dtype(dtype, [&](auto t) {
+      using T = typename decltype(t)::type;
+      dim3 grid(ceil_div(N, 256), C, B);
+      group_points_grad_csr_kernel<T><<<grid, 256, 0, stream>>>(static_cast<const T*>(grad_out), csr_off, csr_ent, C,
+                                                                N, M, K, static_cast<T*>(grad_points));
+      CL3D_LAUNCHED(1);
+      return check_launch("group_points_grad_csr_kernel");
+    });
+  }
   // no atomics on 16-bit types: a 16-bit gradient is accumulated in fp32 and converted once
   float* gp = dtype == CL3D_DTYPE_F32 ? static_cast<float*>(grad_points) : acc;
   const size_t n = (size_t)B * C * N;

@@ -3,7 +3,8 @@
 //   cl3d_ball_query_algo  bit-exact replacement of the reference's masked_ordered_ball_query
 //                         (/root/reference/pytorch/ops/pt_custom_ops/_ext_src/src/masked_ordered_ball_query_gpu.cu:11-96)
 //   cl3d_nearest_query    bit-exact replacement of masked_nearest_query (masked_nearest_query_gpu.cu:8-62)
-//   cl3d_build_csr        transposed neighbour lists for the gather-form backward kernels
+//   cl3d_build_csr        transposed neighbour lists for the gather-form backward kernels (arrival order, or
+//                         ascending entry order with `deterministic`)
 //
 // The reference scans ALL support points per query on B thread blocks.  Here the support cloud is binned
 // into a uniform grid (cell edge >= radius, counting sort, points stored as float4 {x,y,z,index} in cell
@@ -12,6 +13,7 @@
 // (first 3K in-radius points by index, nearest-overwrite rule, stable sort by distance, cyclic padding);
 // that rule is reproduced on the candidate set with 64-bit keys (d2 bits << 32 | index), which order
 // exactly like the reference's stable sort because candidates are unique in index.
+#include <limits.h>
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -968,6 +970,117 @@ __global__ void csr_place_kernel(const int* __restrict__ idx, const int* __restr
   ent[(size_t)b * M * K + off[(size_t)b * (N + 1) + idx[g]] + rank[g]] = (int)e;
 }
 
+// ---------------------------------------------------------------------------------------------
+// canonical list order (deterministic mode): the lists above are filled in atomic arrival order; these two passes
+// rewrite each list from a scratch copy in ascending entry order q*K + k, the order a serial fill would give.
+// Entries of a list are unique, so an entry's place is the number of smaller entries in its list.
+// ---------------------------------------------------------------------------------------------
+constexpr int kCanonWarpMax = 1024;  // longest list one warp ranks (len^2/32 compares per lane); longer: grid pass
+constexpr int kCanonTile = 2048;     // list tile the grid pass stages in shared memory
+
+// one warp per list; lists longer than kCanonWarpMax are queued for csr_canon_long_kernel
+__global__ void __launch_bounds__(256) csr_canon_warp_kernel(const int* __restrict__ off, const int* __restrict__ src,
+                                                             int B, int N, int M, int K, int* __restrict__ ent,
+                                                             int* __restrict__ long_cnt, int* __restrict__ long_list) {
+  const long long gw = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (gw >= (long long)B * N) return;
+  const int lane = threadIdx.x & 31;
+  const int b = (int)(gw / N), j = (int)(gw - (long long)b * N);
+  const int o0 = off[(size_t)b * (N + 1) + j];
+  const int len = off[(size_t)b * (N + 1) + j + 1] - o0;
+  if (len > kCanonWarpMax) {
+    if (lane == 0) long_list[atomicAdd(long_cnt, 1)] = (int)gw;
+    return;
+  }
+  const int* s = src + (size_t)b * M * K + o0;
+  int* d = ent + (size_t)b * M * K + o0;
+  if (len <= 32) {  // the common case: one entry per lane, ranked against the others through shuffles
+    const int v = lane < len ? s[lane] : INT_MAX;
+    int r = 0;
+    for (int t = 0; t < len; ++t) r += __shfl_sync(0xffffffffu, v, t) < v ? 1 : 0;
+    if (lane < len) d[r] = v;
+    return;
+  }
+  for (int base = 0; base < len; base += 64) {
+    const int i0 = base + lane, i1 = base + 32 + lane;
+    const int v0 = i0 < len ? s[i0] : INT_MAX, v1 = i1 < len ? s[i1] : INT_MAX;
+    int r0 = 0, r1 = 0;
+#pragma unroll 4
+    for (int t = 0; t < len; ++t) {
+      const int v = s[t];
+      r0 += v < v0 ? 1 : 0;
+      r1 += v < v1 ? 1 : 0;
+    }
+    if (i0 < len) d[r0] = v0;
+    if (i1 < len) d[r1] = v1;
+  }
+}
+
+// the queued long lists (coincident points, or isolated and padded queries filling all K slots with one point), one
+// at a time with every thread of the grid: thread t ranks entries t, t + T, ... against the list staged in tiles
+__global__ void __launch_bounds__(256) csr_canon_long_kernel(const int* __restrict__ off, const int* __restrict__ src,
+                                                             int N, int M, int K, int* __restrict__ ent,
+                                                             const int* __restrict__ long_cnt,
+                                                             const int* __restrict__ long_list) {
+  __shared__ int s_t[kCanonTile];
+  const int nl = *long_cnt;
+  const int T = gridDim.x * blockDim.x;
+  for (int l = 0; l < nl; ++l) {
+    const int gw = long_list[l];
+    const int b = gw / N, j = gw - b * N;
+    const int o0 = off[(size_t)b * (N + 1) + j];
+    const int len = off[(size_t)b * (N + 1) + j + 1] - o0;
+    const int* s = src + (size_t)b * M * K + o0;
+    int* d = ent + (size_t)b * M * K + o0;
+    for (int base = blockIdx.x * blockDim.x; base < len; base += T) {  // CTA-uniform bounds
+      const int i = base + threadIdx.x;
+      const int v = i < len ? s[i] : INT_MAX;
+      int r = 0;
+      for (int t0 = 0; t0 < len; t0 += kCanonTile) {
+        const int n = min(kCanonTile, len - t0);
+        __syncthreads();
+        for (int t = threadIdx.x; t < n; t += blockDim.x) s_t[t] = s[t0 + t];
+        __syncthreads();
+#pragma unroll 8
+        for (int t = 0; t < n; ++t) r += s_t[t] < v ? 1 : 0;
+      }
+      if (i < len) d[r] = v;
+    }
+  }
+}
+
+// scratch of the canonical pass behind a caller's workspace: the arrival-order copy, the long-list queue, its count
+static size_t canon_workspace_bytes(int B, int N, int M, int K) {
+  const size_t b = (size_t)(B > 0 ? B : 1);
+  return align_up(sizeof(int) * b * (size_t)(M > 0 ? M : 1) * (size_t)K, 256) +
+         align_up(sizeof(int) * b * (size_t)N, 256) + 256;
+}
+
+struct CanonScratch {
+  int* src;
+  int* long_list;
+  int* long_cnt;
+};
+
+static CanonScratch canon_scratch(void* w, int B, int N, int M, int K) {
+  CanonScratch c;
+  c.src = (int*)w;
+  c.long_list = (int*)((unsigned char*)w + align_up(sizeof(int) * (size_t)B * (size_t)M * (size_t)K, 256));
+  c.long_cnt = (int*)((unsigned char*)c.long_list + align_up(sizeof(int) * (size_t)B * (size_t)N, 256));
+  return c;
+}
+
+// the lists in c.src (arrival order) -> ent (ascending entries); sizes only, so a captured graph replays it
+static void canon_lists(const int* off, const CanonScratch& c, int B, int N, int M, int K, int* ent,
+                        cudaStream_t stream) {
+  cudaMemsetAsync(c.long_cnt, 0, sizeof(int), stream);
+  const long long lists = (long long)B * N;
+  csr_canon_warp_kernel<<<(unsigned)((lists + 7) / 8), 256, 0, stream>>>(off, c.src, B, N, M, K, ent, c.long_cnt,
+                                                                         c.long_list); CL3D_LAUNCHED(1);
+  csr_canon_long_kernel<<<2 * sm_count(), 256, 0, stream>>>(off, c.src, N, M, K, ent, c.long_cnt, c.long_list);
+  CL3D_LAUNCHED(1);
+}
+
 }  // namespace cl3d
 
 // =================================================================================================
@@ -1002,21 +1115,22 @@ extern "C" int cl3d_ball_query_algo(const float* query_xyz, const float* support
                          workspace, workspace_bytes, algo, nullptr, nullptr, 0, (cudaStream_t)stream_);
 }
 
-extern "C" size_t cl3d_ball_query_csr_workspace_bytes(int B, int N, int M, int K) {
+extern "C" size_t cl3d_ball_query_csr_workspace_bytes(int B, int N, int M, int K, int deterministic) {
   return cl3d_ball_query_workspace_bytes(B, N, M, K) + align_up(sizeof(int) * (size_t)(B > 0 ? B : 1) * (size_t)N, 256) +
-         align_up(sizeof(int) * (size_t)(B > 0 ? B : 1) * (size_t)(M > 0 ? M : 1) * (size_t)K, 256);
+         align_up(sizeof(int) * (size_t)(B > 0 ? B : 1) * (size_t)(M > 0 ? M : 1) * (size_t)K, 256) +
+         (deterministic ? canon_workspace_bytes(B, N, M, K) : 0);
 }
 
 extern "C" int cl3d_ball_query_csr(const float* query_xyz, const float* support_xyz, const int* query_mask,
                                    const int* support_mask, int B, int N, int M, float radius, int K, int* idx,
                                    int* idx_mask, int* ncount, int all_slots, int* csr_off, int* csr_ent,
-                                   void* workspace, size_t workspace_bytes, int algo, int phases,
+                                   void* workspace, size_t workspace_bytes, int algo, int phases, int deterministic,
                                    cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(phases >= 1 && phases <= 3, "cl3d_ball_query_csr: phases is a mask of 1 (search) | 2 (lists)");
   CL3D_REQUIRE(csr_off && csr_ent && ncount, "cl3d_ball_query_csr: null pointer");
   CL3D_REQUIRE(B >= 0 && N >= 1 && M >= 0 && K >= 1, "cl3d_ball_query_csr: bad sizes");
-  if (workspace_bytes < cl3d_ball_query_csr_workspace_bytes(B, N, M, K) || !workspace) {
+  if (workspace_bytes < cl3d_ball_query_csr_workspace_bytes(B, N, M, K, deterministic) || !workspace) {
     set_error("cl3d_ball_query_csr: workspace too small");
     return CL3D_ERR_WORKSPACE;
   }
@@ -1036,8 +1150,11 @@ extern "C" int cl3d_ball_query_csr(const float* query_xyz, const float* support_
   csr_scan_kernel<<<B, 1024, 0, stream>>>(N, cnt, csr_off, nullptr); CL3D_LAUNCHED(1);
   const long long ents = (long long)M * K;
   if (ents > 0) {
-    csr_place_kernel<<<dim3((unsigned)((ents + 255) / 256), B), 256, 0, stream>>>(idx, ncount, rank, csr_off, N, M, K,
-                                                                                  all_slots ? 1 : 0, csr_ent); CL3D_LAUNCHED(1);
+    const CanonScratch c =
+        canon_scratch((unsigned char*)rank + align_up(sizeof(int) * (size_t)B * M * K, 256), B, N, M, K);
+    csr_place_kernel<<<dim3((unsigned)((ents + 255) / 256), B), 256, 0, stream>>>(
+        idx, ncount, rank, csr_off, N, M, K, all_slots ? 1 : 0, deterministic ? c.src : csr_ent); CL3D_LAUNCHED(1);
+    if (deterministic) canon_lists(csr_off, c, B, N, M, K, csr_ent, stream);
   }
   return check_launch("ball query + transposed lists");
 }
@@ -1157,18 +1274,18 @@ extern "C" int cl3d_nearest_query(const float* query_xyz, const float* support_x
   return check_launch("nearest_query_grid_kernel");
 }
 
-extern "C" size_t cl3d_csr_workspace_bytes(int B, int N, int M, int K) {
-  (void)M;
-  (void)K;
-  return align_up(sizeof(int) * (size_t)(B > 0 ? B : 1) * (size_t)(N > 0 ? N : 1), 256) * 2;
+extern "C" size_t cl3d_csr_workspace_bytes(int B, int N, int M, int K, int deterministic) {
+  return align_up(sizeof(int) * (size_t)(B > 0 ? B : 1) * (size_t)(N > 0 ? N : 1), 256) * 2 +
+         (deterministic ? canon_workspace_bytes(B, N > 0 ? N : 1, M, K) : 0);
 }
 
 extern "C" int cl3d_build_csr(const int* idx, const int* ncount, int B, int N, int M, int K, int* csr_off,
-                              int* csr_ent, void* workspace, size_t workspace_bytes, cl3d_stream_t stream_) {
+                              int* csr_ent, void* workspace, size_t workspace_bytes, int deterministic,
+                              cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(B >= 0 && N >= 1 && M >= 0 && K >= 1, "cl3d_build_csr: bad sizes");
   CL3D_REQUIRE(idx && ncount && csr_off && csr_ent, "cl3d_build_csr: null pointer");
-  if (workspace_bytes < cl3d_csr_workspace_bytes(B, N, M, K) || !workspace) {
+  if (workspace_bytes < cl3d_csr_workspace_bytes(B, N, M, K, deterministic) || !workspace) {
     set_error("cl3d_build_csr: workspace too small");
     return CL3D_ERR_WORKSPACE;
   }
@@ -1182,7 +1299,10 @@ extern "C" int cl3d_build_csr(const int* idx, const int* ncount, int B, int N, i
   }
   csr_scan_kernel<<<B, 1024, 0, stream>>>(N, cnt, csr_off, cursor); CL3D_LAUNCHED(1);
   if (ents > 0) {
-    csr_fill_kernel<<<dim3((unsigned)((ents + 255) / 256), B), 256, 0, stream>>>(idx, ncount, N, M, K, cursor, csr_ent); CL3D_LAUNCHED(1);
+    const CanonScratch c = canon_scratch((unsigned char*)cursor + align_up(sizeof(int) * (size_t)B * N, 256), B, N, M, K);
+    csr_fill_kernel<<<dim3((unsigned)((ents + 255) / 256), B), 256, 0, stream>>>(
+        idx, ncount, N, M, K, cursor, deterministic ? c.src : csr_ent); CL3D_LAUNCHED(1);
+    if (deterministic) canon_lists(csr_off, c, B, N, M, K, csr_ent, stream);
   }
   return check_launch("csr kernels");
 }

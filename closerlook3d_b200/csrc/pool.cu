@@ -6,7 +6,8 @@
 //           coalesced loads; max over ALL K slots (the reference ignores masks here; cyclic padding duplicates
 //           cannot change a max), first arg-max slot kept (max_pool2d's tie rule) for the backward.
 // backward: grad_f[b, c, idx[b,q,arg]] += grad_out[b,c,q]  -- one fp32 red.add row per query into a zeroed
-//           point-major buffer (the reference scatters K times as many atomics through group_points_grad).
+//           point-major buffer (the reference scatters K times as many atomics through group_points_grad); or, given
+//           the transposed lists of idx, the same sum gathered per support point in list order (deterministic mode).
 #include "common.cuh"
 
 namespace cl3d {
@@ -112,6 +113,37 @@ __global__ void __launch_bounds__(256) gather_max_bwd_kernel(const T* __restrict
   }
 }
 
+// gather form over the transposed lists of idx (all K slots, cl3d_build_csr): one warp per support point j, lane =
+// channel; grad_pm[b,j,c] = sum over the list's entries q*K + k with arg[b,q,c] == k of grad_out[b,c,q], in list
+// order, so canonical lists give the same bits on every run.  Every row is written, padded channels with 0.
+template <typename T>
+__global__ void __launch_bounds__(256) gather_max_bwd_csr_kernel(const T* __restrict__ grad_out,
+                                                                 const unsigned char* __restrict__ arg,
+                                                                 const int* __restrict__ csr_off,
+                                                                 const int* __restrict__ csr_ent, int B, int N, int M,
+                                                                 int K, int C, int Cp, float* __restrict__ grad_pm) {
+  const long long gw = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (gw >= (long long)B * N) return;
+  const int lane = threadIdx.x & 31;
+  const int b = (int)(gw / N), j = (int)(gw - (long long)b * N);
+  const int o0 = csr_off[(size_t)b * (N + 1) + j], o1 = csr_off[(size_t)b * (N + 1) + j + 1];
+  const int* ent = csr_ent + (size_t)b * M * K;
+  const unsigned char* a = arg + (size_t)b * M * Cp;
+  float* row = grad_pm + ((size_t)b * N + j) * Cp;
+  for (int c = lane; c < Cp; c += 32) {
+    float acc = 0.f;
+    if (c < C) {
+      const T* g = grad_out + ((size_t)b * C + c) * M;
+      for (int p = o0; p < o1; ++p) {
+        const int e = ent[p];
+        const int q = e / K;
+        if (a[(size_t)q * Cp + c] == e - q * K) acc += load_f32(g + q);
+      }
+    }
+    row[c] = acc;
+  }
+}
+
 template <int CI, typename T>
 static int launch_pool_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, int Cp, T* out,
                            unsigned char* arg, cudaStream_t stream) {
@@ -151,13 +183,25 @@ extern "C" int cl3d_gather_max_fwd(const float* feat_pm, const int* idx, int B, 
 }
 
 extern "C" int cl3d_gather_max_bwd(const void* grad_out, int dtype, const int* idx, const unsigned char* arg, int B,
-                                   int N, int M, int K, int C, float* grad_pm, cl3d_stream_t stream_) {
+                                   int N, int M, int K, int C, const int* csr_off, const int* csr_ent, float* grad_pm,
+                                   cl3d_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   CL3D_REQUIRE(grad_out && idx && arg && grad_pm && B >= 0 && N >= 1 && M >= 1 && K >= 1 && C >= 1,
                "cl3d_gather_max_bwd: bad arguments");
+  CL3D_REQUIRE(!csr_off == !csr_ent, "cl3d_gather_max_bwd: csr_off and csr_ent are both given or both NULL");
   CL3D_REQUIRE_DTYPE(dtype, "cl3d_gather_max_bwd");
   if (B == 0) return CL3D_OK;
   const int Cp = padded_channels(C);
+  if (csr_off) {
+    return with_dtype(dtype, [&](auto t) {
+      using T = typename decltype(t)::type;
+      const long long rows = (long long)B * N;
+      gather_max_bwd_csr_kernel<T><<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(
+          static_cast<const T*>(grad_out), arg, csr_off, csr_ent, B, N, M, K, C, Cp, grad_pm);
+      CL3D_LAUNCHED(1);
+      return check_launch("gather_max_bwd_csr_kernel");
+    });
+  }
   cudaMemsetAsync(grad_pm, 0, sizeof(float) * (size_t)B * N * Cp, stream);
   const size_t smem = (size_t)32 * (C + 1) * sizeof(float);
   return with_dtype(dtype, [&](auto t) {

@@ -24,6 +24,10 @@
 //                           cnt_j and sum_e a'[q_e]  -> one row gather, 2 instructions per element, no atomics
 //   pwmlp_bwd_query_kernel  thread per (query, 4 channels), no K loop: d/da' in closed form from the saved S,
 //                           d/dA[j_0] as one red.global.add.v4.f32, the arg-max slot's sc*dz, d/dWp partials
+// deterministic mode (torch's flag): the query pass stores d/da' point-major instead, and
+//   pwmlp_bwd_gather_det_kernel  support-major over the canonical all-slots lists: each grad_ab row (d/dA from the
+//                           slot-0 entries, d/dT from the dense term and the arg-max entries) summed in list order
+//                           and stored once -- in eval mode too (no dense term there)
 #include <mutex>
 
 #include "common.cuh"
@@ -385,7 +389,10 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_bwd_dense_kernel(const Pw
 // Layers wider than 4 * kPWQGroups channels split their channel groups over blockIdx.y (one slice per CTA).
 constexpr int kPWQPT = 8;        // queries per thread
 constexpr int kPWQGroups = 256;  // channel groups of 4 per CTA slice (= the block size when ny = 1)
-__global__ void __launch_bounds__(256) pwmlp_bwd_query_kernel(const PwArgs a, long long nqueries /* B*M */) {
+// DET (deterministic mode): no reductions into grad_ab; da' is stored point-major in da_pm (B,M,Cop) and
+// pwmlp_bwd_gather_det_kernel builds every grad_ab row from the canonical lists.
+template <bool DET>
+__device__ __forceinline__ void pwmlp_bwd_query_body(const PwArgs& a, long long nqueries, float* __restrict__ da_pm) {
   extern __shared__ float s_dw[];  // [ny][3][Cop]
   const int ngroups = a.Cop >> 2;
   const int nx = ngroups < kPWQGroups ? ngroups : kPWQGroups, ny = blockDim.x / nx;
@@ -431,15 +438,20 @@ __global__ void __launch_bounds__(256) pwmlp_bwd_query_kernel(const PwArgs a, lo
 #pragma unroll
       for (int t = 0; t < 4; ++t) {
         da[t] = (c4 + t < a.Cout) ? dzv[t] - fK * c1[t] - c2[t] * fmaf(fK, apv[t] - mean[t], sbv[t]) : 0.f;
-        if (dzv[t] != 0.f && c4 + t < a.Cout)
+        if (!DET && dzv[t] != 0.f && c4 + t < a.Cout)
           atomicAdd(gab + (size_t)irow[ksv[t]] * 2 * a.Cop + a.Cop + c4 + t, sg[t] * dzv[t]);
         dw[0][t] = fmaf(-da[t], qx, dw[0][t]);
         dw[1][t] = fmaf(-da[t], qy, dw[1][t]);
         dw[2][t] = fmaf(-da[t], qz, dw[2][t]);
       }
-      float* pa = gab + (size_t)j0 * 2 * a.Cop + c4;
-      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(pa), "f"(da[0]), "f"(da[1]), "f"(da[2]), "f"(da[3])
-                   : "memory");
+      if (DET) {
+        *reinterpret_cast<float4*>(da_pm + o) = make_float4(da[0], da[1], da[2], da[3]);
+      } else {
+        float* pa = gab + (size_t)j0 * 2 * a.Cop + c4;
+        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(pa), "f"(da[0]), "f"(da[1]), "f"(da[2]),
+                     "f"(da[3])
+                     : "memory");
+      }
     }
     if (active)
 #pragma unroll
@@ -455,6 +467,90 @@ __global__ void __launch_bounds__(256) pwmlp_bwd_query_kernel(const PwArgs a, lo
     float t = 0.f;
     for (int yy = 0; yy < ny; ++yy) t += s_dw[((size_t)yy * 3 + s3) * a.Cop + c];
     a.partial[((size_t)blockIdx.x * 3 + s3) * a.Cout + c] = t;
+  }
+}
+
+__global__ void __launch_bounds__(256) pwmlp_bwd_query_kernel(const PwArgs a, long long nqueries /* B*M */) {
+  pwmlp_bwd_query_body<false>(a, nqueries, nullptr);
+}
+
+__global__ void __launch_bounds__(256) pwmlp_bwd_query_det_kernel(const PwArgs a, long long nqueries,
+                                                                  float* __restrict__ da_pm) {
+  pwmlp_bwd_query_body<true>(a, nqueries, da_pm);
+}
+
+// Deterministic mode: support-major over the canonical all-slots lists of point j (ascending q*K + k), every grad_ab
+// row built in registers and stored once (no zero-fill, no atomics):
+//   grad_A[j] = sum over entries with k == 0 of da'[q]
+//   grad_T[j] = sgn * ( dense term of pwmlp_bwd_dense_kernel (training only)
+//                       + sum over entries with karg[q][c] == k of sc*dz[q][c] )
+template <int CI>
+__global__ void __launch_bounds__(kPWWarps * 32) pwmlp_bwd_gather_det_kernel(const PwArgs a,
+                                                                             const float* __restrict__ da_pm) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int c0 = blockIdx.y * 32 * CI;
+  const int chunkC = min(32 * CI, a.Cop - c0);
+  const bool training = a.inv_count != 0.f;
+  float c1[CI], c2[CI], sg[CI];
+#pragma unroll
+  for (int i = 0; i < CI; ++i) {
+    const int c = c0 + lane + 32 * i;
+    const bool ok = c < a.Cout;
+    const float invstd = ok ? a.stats[a.Cout + c] : 0.f;
+    const float sc = ok ? invstd * a.gamma[c] : 0.f;
+    c1[i] = ok ? sc * a.dgb[a.Cout + c] * a.inv_count : 0.f;
+    c2[i] = ok ? sc * invstd * a.dgb[c] * a.inv_count : 0.f;
+    sg[i] = ok ? a.sgn[c] : 1.f;
+  }
+  const int per_cloud = (a.N + kPWTile - 1) / kPWTile;
+  for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
+    const int b = tile / per_cloud;
+    const int j0 = (tile % per_cloud) * kPWTile;
+    const size_t base = (size_t)b * a.M * a.Cop + c0 + lane;
+    const float* aq = a.aq + base;
+    const float* dab = da_pm + base;
+    const float* dzb = a.dzs_pm + base;
+    const unsigned char* kb = a.karg + base;
+    float a0[CI];
+#pragma unroll
+    for (int i = 0; i < CI; ++i) a0[i] = lane + 32 * i < chunkC ? __ldg(aq + 32 * i) : 0.f;
+    const int* off = a.csr_off + (size_t)b * (a.N + 1);
+    const int* ent = a.csr_ent + (size_t)b * a.M * a.K;
+    for (int jl = warp; jl < kPWTile; jl += kPWWarps) {
+      const int j = j0 + jl;
+      if (j >= a.N) continue;
+      const int e0 = off[j], e1 = off[j + 1];
+      float acc[CI], gA[CI], gT[CI];
+#pragma unroll
+      for (int i = 0; i < CI; ++i) acc[i] = gA[i] = gT[i] = 0.f;
+      for (int p = e0; p < e1; ++p) {
+        const int e = ent[p];
+        const int q = e / a.K, k = e - q * a.K;
+        const size_t o = (size_t)q * a.Cop;
+#pragma unroll
+        for (int i = 0; i < CI; ++i) {
+          if (lane + 32 * i >= chunkC) continue;
+          if (training) acc[i] += __ldg(aq + o + 32 * i) - a0[i];
+          if (k == 0) gA[i] += __ldg(dab + o + 32 * i);
+          if (kb[o + 32 * i] == k) gT[i] += __ldg(dzb + o + 32 * i);
+        }
+      }
+      const float cnt = (float)(e1 - e0);
+      const float* trow = a.ab_pm + ((size_t)b * a.N + j) * 2 * a.Cop + a.Cop + c0 + lane;
+      float* grow = a.grad_ab_pm + ((size_t)b * a.N + j) * 2 * a.Cop + c0 + lane;
+#pragma unroll
+      for (int i = 0; i < CI; ++i) {
+        const int c = c0 + lane + 32 * i;
+        if (lane + 32 * i >= chunkC) continue;
+        float dbv = 0.f;
+        if (training && c < a.Cout) {
+          const float bv = sg[i] * __ldg(trow + 32 * i);
+          dbv = -cnt * c1[i] - c2[i] * (acc[i] + cnt * ((bv + a0[i]) - __ldg(a.stats + c)));
+        }
+        grow[32 * i] = gA[i];
+        grow[a.Cop + 32 * i] = sg[i] * (dbv + gT[i]);
+      }
+    }
   }
 }
 
@@ -551,6 +647,15 @@ static int launch_pw_bwd(const PwArgs& a, int ntiles_n, int gx, cudaStream_t str
   return check_launch("pwmlp_bwd_dense_kernel");
 }
 
+template <int CI>
+static int launch_pw_bwd_det(const PwArgs& a, const float* da_pm, int ntiles_n, int gx, cudaStream_t stream) {
+  PwArgs d = a;
+  d.ntiles = ntiles_n;
+  pwmlp_bwd_gather_det_kernel<CI><<<dim3(gx, ceil_div(a.Cop, 32 * CI)), kPWWarps * 32, 0, stream>>>(d, da_pm);
+  CL3D_LAUNCHED(1);
+  return check_launch("pwmlp_bwd_gather_det_kernel");
+}
+
 static int pw_dense_grid(int ntiles_n) {
   int gx = persistent_grid_cap();
   return gx > ntiles_n ? ntiles_n : gx;
@@ -639,12 +744,13 @@ extern "C" int cl3d_pwmlp_fwd_out(const float* ysel, const float* save_stats, co
   });
 }
 
-extern "C" size_t cl3d_pwmlp_bwd_scratch_floats(int B, int N, int M, int Cout) {
+extern "C" size_t cl3d_pwmlp_bwd_scratch_floats(int B, int N, int M, int Cout, int deterministic) {
   const int Cop = padded_channels(Cout);
   (void)N;
   const size_t ntm = (size_t)B * ceil_div(M, kPWTile), gq = (size_t)pw_query_grid(B, M, Cop);
   const size_t part = (ntm * 2 > gq * 3 ? ntm * 2 : gq * 3) * (size_t)Cout;
-  return part + (size_t)B * M * Cop + 64;
+  // deterministic: da' point-major (B*M*Cop) behind sc*dz
+  return part + (size_t)B * M * Cop * (deterministic ? 2 : 1) + 64 + (deterministic ? 64 : 0);
 }
 
 // fork/join events of cl3d_pwmlp_bwd: a small per-device ring of event sets, so that several calls can be in
@@ -677,12 +783,13 @@ extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta
                               const int* idx, const int* csr_off, const int* csr_ent, const float* ysel,
                               const float* aq, const float* sq, const unsigned char* karg, const float* save_stats,
                               const float* gamma, int B, int N, int M, int K, int Cout, float radius, int training,
-                              float* scratch, float* dgamma_dbeta, float* grad_ab_pm, float* grad_wp,
-                              cl3d_stream_t stream_, cl3d_stream_t side_stream_) {
+                              int deterministic, float* scratch, float* dgamma_dbeta, float* grad_ab_pm,
+                              float* grad_wp, cl3d_stream_t stream_, cl3d_stream_t side_stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   // With a side stream the zero-fill of grad_ab and the latency-bound query pass run beside the statistics and
   // the support-major gather (fork/join with events: capturable into a CUDA graph); without one, in order.
-  cudaStream_t side = side_stream_ ? (cudaStream_t)side_stream_ : stream;
+  // Deterministic mode runs in order on `stream`: its gather pass reads the query pass's da'.
+  cudaStream_t side = side_stream_ && !deterministic ? (cudaStream_t)side_stream_ : stream;
   const bool forked = side != stream;
   PwEvents* ev = forked ? pw_events() : nullptr;
   if (forked && !ev) return CL3D_ERR_LAUNCH;
@@ -690,7 +797,8 @@ extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta
   CL3D_REQUIRE(grad_out && beta && ab_pm && wp && sgn && query_xyz && support_xyz && idx && ysel && aq && sq &&
                    karg && save_stats && gamma && scratch && dgamma_dbeta && grad_ab_pm && grad_wp,
                "cl3d_pwmlp_bwd: null pointer");
-  CL3D_REQUIRE(!training || (csr_off && csr_ent), "cl3d_pwmlp_bwd: training mode needs the all-slots CSR lists");
+  CL3D_REQUIRE((!training && !deterministic) || (csr_off && csr_ent),
+               "cl3d_pwmlp_bwd: training or deterministic mode needs the all-slots CSR lists");
   CL3D_REQUIRE(B >= 0 && N >= 1 && M >= 1 && K >= 1 && K <= 255 && Cout >= 1, "cl3d_pwmlp_bwd: bad sizes");
   if (B == 0) return CL3D_OK;
   const int ntiles = B * ceil_div(M, kPWTile);
@@ -703,11 +811,12 @@ extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta
   float* partial = scratch;
   float* dzs_pm = scratch + ((part + 63) / 64) * 64;
   const size_t smem_s = (size_t)kPWTile * (Cop + 1) * sizeof(float);
+  float* da_pm = dzs_pm + (((size_t)B * M * Cop + 63) / 64) * 64;  // deterministic mode only
   if (forked) {
     cudaEventRecord(ev->start, stream);
     cudaStreamWaitEvent(side, ev->start, 0);
   }
-  cudaMemsetAsync(grad_ab_pm, 0, sizeof(float) * (size_t)B * N * 2 * Cop, side);
+  if (!deterministic) cudaMemsetAsync(grad_ab_pm, 0, sizeof(float) * (size_t)B * N * 2 * Cop, side);
   if (forked) cudaEventRecord(ev->zeroed, side);
   with_dtype(dtype, [&](auto t) {
     using TG = typename decltype(t)::type;
@@ -741,6 +850,22 @@ extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta
   // pass) and the dense support-major pass would add exact zeros, so it is not launched
   a.inv_count = training ? 1.0f / (float)((double)B * M * K) : 0.f;
   a.ntiles = ntiles;
+  if (deterministic) {
+    const int nx = Cop / 4 < kPWQGroups ? Cop / 4 : kPWQGroups, ny = 256 / nx;
+    pwmlp_bwd_query_det_kernel<<<dim3(gqy, ceil_div(Cop / 4, nx)), ny * nx, (size_t)ny * 3 * Cop * sizeof(float),
+                                 stream>>>(a, (long long)B * M, da_pm);
+    CL3D_LAUNCHED(1);
+    rc = check_launch("pwmlp_bwd_query_det_kernel");
+    if (rc) return rc;
+    rc = cl3d_reduce_partials(partial, gqy, 3 * Cout, grad_wp, stream_);
+    if (rc) return rc;
+    switch (pw_ci(Cop)) {
+      case 1: return launch_pw_bwd_det<1>(a, da_pm, ntn, gx, stream);
+      case 2: return launch_pw_bwd_det<2>(a, da_pm, ntn, gx, stream);
+      case 3: return launch_pw_bwd_det<3>(a, da_pm, ntn, gx, stream);
+      default: return launch_pw_bwd_det<4>(a, da_pm, ntn, gx, stream);
+    }
+  }
   if (training) {
     switch (pw_ci(Cop)) {
       case 1: rc = launch_pw_bwd<1>(a, ntn, gx, stream); break;

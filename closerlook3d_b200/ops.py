@@ -60,6 +60,13 @@ def no_autocast(fn):
     return call
 
 
+def deterministic_mode(deterministic=None):
+    """None -> torch's flag (torch.use_deterministic_algorithms) at the time of the call.  Under it the transposed
+    neighbour lists are built in canonical order (ascending q*K + k) and the scatters take their gather forms, so
+    every fused operator gives the same bits on every run."""
+    return torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
+
+
 def padded_channels(C):
     return (C + 7) & ~7
 
@@ -74,14 +81,14 @@ def _empty_pm(B, N, W, device):
 
 @_on_device
 def ball_query(query_xyz, support_xyz, query_mask, support_mask, radius, nsample, want_mask=True, want_ncount=True,
-               algo=0, csr=None, after_search=None, out=None):
+               algo=0, csr=None, after_search=None, out=None, deterministic=None):
     """-> (idx (B,M,K) i32, idx_mask (B,M,K) i32 | None, ncount (B,M) i32 | None); bit-exact with the
     reference's masked_ordered_ball_query (masked_ordered_ball_query_gpu.cu:11-96).
     csr = "counted" | "all": also build the transposed lists in the same call (cl3d_ball_query_csr) and return
     (idx, idx_mask, ncount, (csr_off, csr_ent)).  after_search(): called between the search and the list build (the
     caller records its "search done" event there, so consumers of idx do not wait for the lists).
     out: dict of preallocated result tensors (idx, idx_mask, ncount, off, ent -- e.g. batch slices of larger tensors)
-    to write into instead of allocating."""
+    to write into instead of allocating.  deterministic (None: torch's flag): the lists in canonical order."""
     require_cuda(query_xyz, "query_xyz", F32)
     require_cuda(support_xyz, "support_xyz", F32)
     require_cuda(query_mask, "query_mask", I32)
@@ -100,16 +107,17 @@ def ball_query(query_xyz, support_xyz, query_mask, support_mask, radius, nsample
         assert csr in ("counted", "all")
         off = out["off"] if "off" in out else torch.empty(B, N + 1, dtype=I32, device=dev)
         ent = out["ent"] if "ent" in out else torch.empty(B, M * K, dtype=I32, device=dev)
-        wsb = L.cl3d_ball_query_csr_workspace_bytes(B, N, M, K)
+        det = int(deterministic_mode(deterministic))
+        wsb = L.cl3d_ball_query_csr_workspace_bytes(B, N, M, K, det)
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         args = (ptr(query_xyz), ptr(support_xyz), ptr(query_mask), ptr(support_mask), B, N, M, float(radius), K, ptr(idx),
                 ptr(idx_mask), ptr(ncount), 1 if csr == "all" else 0, ptr(off), ptr(ent), ptr(ws), wsb, int(algo))
         if after_search is None:
-            check(L.cl3d_ball_query_csr(*args, 3, stream_ptr()), "cl3d_ball_query_csr")
+            check(L.cl3d_ball_query_csr(*args, 3, det, stream_ptr()), "cl3d_ball_query_csr")
         else:
-            check(L.cl3d_ball_query_csr(*args, 1, stream_ptr()), "cl3d_ball_query_csr (search)")
+            check(L.cl3d_ball_query_csr(*args, 1, det, stream_ptr()), "cl3d_ball_query_csr (search)")
             after_search()
-            check(L.cl3d_ball_query_csr(*args, 2, stream_ptr()), "cl3d_ball_query_csr (lists)")
+            check(L.cl3d_ball_query_csr(*args, 2, det, stream_ptr()), "cl3d_ball_query_csr (lists)")
         return idx, idx_mask, ncount, (off, ent)
     wsb = L.cl3d_ball_query_workspace_bytes(B, N, M, K)
     ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
@@ -139,16 +147,20 @@ def nearest_query(query_xyz, support_xyz, query_mask, support_mask):
 
 
 @_on_device
-def build_csr(idx, ncount, N):
-    """transposed neighbour lists -> (csr_off (B,N+1) i32, csr_ent (B,M*K) i32)"""
+def build_csr(idx, ncount, N, deterministic=None):
+    """transposed neighbour lists -> (csr_off (B,N+1) i32, csr_ent (B,M*K) i32); ncount None = all K slots.
+    deterministic (None: torch's flag): each list in ascending q*K + k instead of atomic arrival order."""
     B, M, K = idx.shape
     dev = idx.device
     L = _lib.lib()
+    if ncount is None:
+        ncount = torch.full((B, M), K, dtype=I32, device=dev)
+    det = int(deterministic_mode(deterministic))
     off = torch.empty(B, N + 1, dtype=I32, device=dev)
     ent = torch.empty(B, M * K, dtype=I32, device=dev)
-    wsb = L.cl3d_csr_workspace_bytes(B, N, M, K)
+    wsb = L.cl3d_csr_workspace_bytes(B, N, M, K, det)
     ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-    check(L.cl3d_build_csr(ptr(idx), ptr(ncount), B, N, M, K, ptr(off), ptr(ent), ptr(ws), wsb, stream_ptr()),
+    check(L.cl3d_build_csr(ptr(idx), ptr(ncount), B, N, M, K, ptr(off), ptr(ent), ptr(ws), wsb, det, stream_ptr()),
           "cl3d_build_csr")
     return off, ent
 
@@ -187,15 +199,20 @@ def group_points(points, idx):
 
 
 @_on_device
-def group_points_grad(grad_out, idx, n):
-    """a 16-bit gradient is accumulated in an fp32 buffer and rounded once"""
+def group_points_grad(grad_out, idx, n, deterministic=None):
+    """a 16-bit gradient is accumulated in fp32 and rounded once.  deterministic (None: torch's flag): gathered
+    over the canonical transposed lists of idx instead of scattered with atomics"""
     dt = require_features(grad_out, "grad_out")
     require_cuda(idx, "idx", I32)
     B, C, M, K = grad_out.shape
     out = torch.empty(B, C, int(n), dtype=grad_out.dtype, device=grad_out.device)
-    acc = torch.empty(B, C, int(n), dtype=F32, device=grad_out.device) if dt else None
-    check(_lib.lib().cl3d_group_points_grad(ptr(grad_out), dt, ptr(idx), B, C, int(n), M, K, ptr(out), ptr(acc),
-                                            stream_ptr()), "cl3d_group_points_grad")
+    off = ent = acc = None
+    if deterministic_mode(deterministic):
+        off, ent = build_csr(idx, None, int(n), deterministic=True)
+    elif dt:
+        acc = torch.empty(B, C, int(n), dtype=F32, device=grad_out.device)
+    check(_lib.lib().cl3d_group_points_grad(ptr(grad_out), dt, ptr(idx), B, C, int(n), M, K, ptr(off), ptr(ent),
+                                            ptr(out), ptr(acc), stream_ptr()), "cl3d_group_points_grad")
     return out
 
 
@@ -390,22 +407,25 @@ def pwmlp_fwd_out(ysel, stats, gamma, beta, dtype=F32):
 
 @_on_device
 def pwmlp_bwd(grad_out, beta, ab_pm, wp, sgn, query_xyz, support_xyz, idx, csr_off, csr_ent, ysel, aq, sq, karg, stats,
-              gamma, radius, side_stream=None, training=True):
+              gamma, radius, side_stream=None, training=True, deterministic=None):
     """grad_out in the features' dtype -> (grad_ab_pm (B,N,2Cop), grad_wp (3,Cout), dgamma (Cout), dbeta (Cout)), fp32;
     the ReLU decision is recomputed from ysel, stats, gamma and beta.  side_stream: a torch stream the library may fork
-    onto (zero-fill + query pass run beside the gather pass), joined before it returns"""
+    onto (zero-fill + query pass run beside the gather pass), joined before it returns.  deterministic (None: torch's
+    flag): no atomics, every grad_ab row gathered from the canonical all-slots lists csr_off / csr_ent (required then,
+    in eval mode too)"""
     dt = require_features(grad_out, "grad_out")
     B, N, C2 = ab_pm.shape
     Cout, M, K = ysel.shape[1], ysel.shape[2], idx.shape[2]
     L = _lib.lib()
     dev = ysel.device
-    partial = _empty_pm(1, 1, L.cl3d_pwmlp_bwd_scratch_floats(B, N, M, Cout), dev)  # partial sums + sc*dz rows
+    det = int(deterministic_mode(deterministic))
+    partial = _empty_pm(1, 1, L.cl3d_pwmlp_bwd_scratch_floats(B, N, M, Cout, det), dev)  # partials + sc*dz (+ da') rows
     dgb = torch.empty(2, Cout, dtype=F32, device=dev)
     grad_ab = torch.empty(B, N, C2, dtype=F32, device=dev)
     grad_wp = torch.empty(3, Cout, dtype=F32, device=dev)
     check(L.cl3d_pwmlp_bwd(ptr(grad_out), dt, ptr(beta), ptr(ab_pm), ptr(wp), ptr(sgn), ptr(query_xyz), ptr(support_xyz), ptr(idx),
                            ptr(csr_off), ptr(csr_ent), ptr(ysel), ptr(aq), ptr(sq), ptr(karg), ptr(stats), ptr(gamma),
-                           B, N, M, K, Cout, float(radius), int(bool(training)), ptr(partial), ptr(dgb), ptr(grad_ab),
+                           B, N, M, K, Cout, float(radius), int(bool(training)), det, ptr(partial), ptr(dgb), ptr(grad_ab),
                            ptr(grad_wp),
                            stream_ptr(), ctypes.c_void_p(side_stream.cuda_stream) if side_stream is not None else None),
           "cl3d_pwmlp_bwd")
@@ -449,14 +469,18 @@ def gather_max(features, idx):
 
 
 @_on_device
-def gather_max_grad(grad_out, idx, arg, N):
-    """-> d/dfeatures (B,C,N) in grad_out's dtype (accumulated in fp32, rounded once)"""
+def gather_max_grad(grad_out, idx, arg, N, csr=None, deterministic=None):
+    """-> d/dfeatures (B,C,N) in grad_out's dtype (accumulated in fp32, rounded once).  deterministic (None: torch's
+    flag): gathered over the canonical all-slots lists of idx -- `csr` when the caller has them, else built here"""
     dt = require_features(grad_out, "grad_out")
     B, C, M = grad_out.shape
     K = idx.shape[2]
+    off = ent = None
+    if deterministic_mode(deterministic):
+        off, ent = csr if csr is not None else build_csr(idx, None, N, deterministic=True)
     g_pm = torch.empty(B, N, padded_channels(C), dtype=F32, device=grad_out.device)
-    check(_lib.lib().cl3d_gather_max_bwd(ptr(grad_out), dt, ptr(idx), ptr(arg), B, N, M, K, C, ptr(g_pm),
-                                         stream_ptr()), "cl3d_gather_max_bwd")
+    check(_lib.lib().cl3d_gather_max_bwd(ptr(grad_out), dt, ptr(idx), ptr(arg), B, N, M, K, C, ptr(off), ptr(ent),
+                                         ptr(g_pm), stream_ptr()), "cl3d_gather_max_bwd")
     return to_channel_major(g_pm, C, grad_out.dtype)
 
 

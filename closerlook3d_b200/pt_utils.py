@@ -42,6 +42,7 @@ class NeighborList:
         self.idx, self.ncount, self._idx_mask, self.N = idx, ncount, idx_mask, N
         self._csr = None
         self._csr_all = None
+        self._csr_det = self._csr_all_det = False   # whether each list set is canonical (ops.deterministic_mode)
         self.parts = None          # [(b0, b1, search-done event)] when the batch was searched in parts
         self.event = None
         self._csr_event = None
@@ -58,46 +59,56 @@ class NeighborList:
             raise RuntimeError("idx_mask was not requested for this neighbour list")
         return self._idx_mask
 
-    def _build(self, all_slots):
+    def _build(self, all_slots, det):
+        return ops.build_csr(self.idx, None if all_slots else self.ncount, self.N, deterministic=det)
+
+    def _have(self, all_slots, det):
+        """lists of this kind exist and were built in mode `det` (a change of torch's flag rebuilds them)"""
         if all_slots:
-            full = torch.full_like(self.ncount, self.idx.shape[2])
-            return ops.build_csr(self.idx, full, self.N)
-        return ops.build_csr(self.idx, self.ncount, self.N)
+            return self._csr_all is not None and self._csr_all_det == det
+        return self._csr is not None and self._csr_det == det
+
+    def _set(self, all_slots, det, csr, ev):
+        if all_slots:
+            self._csr_all, self._csr_all_det, self._csr_all_event = csr, det, ev
+        else:
+            self._csr, self._csr_det, self._csr_event = csr, det, ev
 
     def prefetch_csr(self, all_slots=False):
         """enqueue the transposed-list build on the side stream right behind the search"""
-        if (self._csr_all if all_slots else self._csr) is not None:
+        det = ops.deterministic_mode()
+        if self._have(all_slots, det):
             return
         side = _side_stream(self.idx.device)
         if self.event is not None:
             side.wait_event(self.event)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
-            csr = self._build(all_slots)
+            csr = self._build(all_slots, det)
             ev = torch.cuda.Event()
             ev.record(side)
-        if all_slots:
-            self._csr_all, self._csr_all_event = csr, ev
+        self._set(all_slots, det, csr, ev)
+
+    def _lists(self, all_slots):
+        det = ops.deterministic_mode()
+        if not self._have(all_slots, det):
+            self.wait()
+            self._set(all_slots, det, self._build(all_slots, det), None)
         else:
-            self._csr, self._csr_event = csr, ev
+            ev = self._csr_all_event if all_slots else self._csr_event
+            if ev is not None:
+                torch.cuda.current_stream().wait_event(ev)
+        return self._csr_all if all_slots else self._csr
 
     def csr(self):
-        """transposed lists over the COUNTED slots (k < ncount): avg/sum families"""
-        if self._csr is None:
-            self.wait()
-            self._csr = self._build(False)
-        elif self._csr_event is not None:
-            torch.cuda.current_stream().wait_event(self._csr_event)
-        return self._csr
+        """transposed lists over the COUNTED slots (k < ncount): avg/sum families.  Canonical order while torch's
+        deterministic flag is on."""
+        return self._lists(False)
 
     def csr_all_slots(self):
-        """transposed lists over ALL K slots (BatchNorm2d of PointWiseMLP sees every slot)"""
-        if self._csr_all is None:
-            self.wait()
-            self._csr_all = self._build(True)
-        elif self._csr_all_event is not None:
-            torch.cuda.current_stream().wait_event(self._csr_all_event)
-        return self._csr_all
+        """transposed lists over ALL K slots (BatchNorm2d of PointWiseMLP sees every slot; the max-pool and
+        group-points gradients' gather forms)"""
+        return self._lists(True)
 
 
 _SIDE = {}
@@ -150,6 +161,7 @@ def neighbors(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
             return hit[0]
     cache_stats["miss"] += 1
     overlap = overlap_enabled if overlap is None else overlap
+    det = ops.deterministic_mode()
     lists = None
     if overlap:
         cur = torch.cuda.current_stream()
@@ -163,7 +175,7 @@ def neighbors(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
                 ev = torch.cuda.Event()      # search done: idx / ncount final (the forward kernels wait for this one)
                 res = ops.ball_query(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
                                      want_mask=need_mask, want_ncount=True, csr=csr,
-                                     after_search=(lambda: ev.record(side)) if csr else None)
+                                     after_search=(lambda: ev.record(side)) if csr else None, deterministic=det)
                 if not csr:
                     ev.record(side)
                 idx, idx_mask, ncount = res[:3]
@@ -183,7 +195,7 @@ def neighbors(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
                                off=lists[0][b0:b1], ent=lists[1][b0:b1])
                     ops.ball_query(query_xyz[b0:b1], support_xyz[b0:b1], query_mask[b0:b1], support_mask[b0:b1], radius,
                                    nsample, want_mask=need_mask, want_ncount=True, csr=csr, out=out,
-                                   after_search=(lambda e=evh: e.record(side)))
+                                   after_search=(lambda e=evh: e.record(side)), deterministic=det)
                     parts.append((b0, b1, evh))
                 ev = parts[-1][2]            # every part searched (stream order)
             ev_lists = None
@@ -195,16 +207,13 @@ def neighbors(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
         nl.parts = parts
     else:
         res = ops.ball_query(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
-                             want_mask=need_mask, want_ncount=True, csr=csr)
+                             want_mask=need_mask, want_ncount=True, csr=csr, deterministic=det)
         idx, idx_mask, ncount = res[:3]
         lists = res[3] if csr else None
         nl = NeighborList(idx, ncount, idx_mask, support_xyz.shape[1])
     if lists is not None:
         lists_event = ev_lists if overlap else None    # in-order on the current stream without overlap
-        if csr == "all":
-            nl._csr_all, nl._csr_all_event = lists, lists_event
-        else:
-            nl._csr, nl._csr_event = lists, lists_event
+        nl._set(csr == "all", det, lists, lists_event)
     if cache_enabled:
         _CACHE[key] = (nl, (query_xyz, support_xyz, query_mask, support_mask))
         while len(_CACHE) > _CACHE_SIZE:
@@ -343,21 +352,23 @@ class MaskedNearestQueryAndGroup(nn.Module):
 
 
 class _GatherMax(Function):
-    """out[b,c,q] = max_k f[b,c,idx[b,q,k]]  (fused MaskedMaxPool body: pt_utils.py:195-201)"""
+    """out[b,c,q] = max_k f[b,c,idx[b,q,k]]  (fused MaskedMaxPool body: pt_utils.py:195-201); nl = the NeighborList
+    of idx, whose cached all-slots lists the deterministic backward gathers over"""
 
     @staticmethod
     @ops.no_autocast
-    def forward(ctx, features, idx):
+    def forward(ctx, features, idx, nl):
         out, arg = ops.gather_max(features, idx)   # in the features' dtype; the winning slots decide the backward
         ctx.save_for_backward(idx, arg)
-        ctx.N = features.shape[2]
+        ctx.N, ctx.nl = features.shape[2], nl
         return out
 
     @staticmethod
     @ops.no_autocast
     def backward(ctx, grad_out):
         idx, arg = ctx.saved_tensors
-        return ops.gather_max_grad(grad_out.contiguous(), idx, arg, ctx.N), None
+        csr = ctx.nl.csr_all_slots() if ops.deterministic_mode() else None
+        return ops.gather_max_grad(grad_out.contiguous(), idx, arg, ctx.N, csr=csr), None, None
 
 
 class MaskedMaxPool(nn.Module):
@@ -372,7 +383,7 @@ class MaskedMaxPool(nn.Module):
         sub_xyz = sub_xyz.contiguous()
         sub_mask = sub_mask.contiguous()
         nl = neighbors(sub_xyz, xyz, sub_mask, mask, self.radius, self.nsample).wait()
-        sub_features = _GatherMax.apply(features.contiguous(), nl.idx)
+        sub_features = _GatherMax.apply(features.contiguous(), nl.idx, nl)
         return sub_xyz, sub_mask, sub_features
 
 
@@ -389,5 +400,5 @@ class MaskedUpsample(nn.Module):
             return grouping_operation(features, idx)[..., 0].contiguous()
         elif self.mode == 'max':
             nl = neighbors(up_xyz, xyz, up_mask, mask, self.radius, self.nsample).wait()
-            return _GatherMax.apply(features.contiguous(), nl.idx)
+            return _GatherMax.apply(features.contiguous(), nl.idx, nl)
         raise NotImplementedError(f"mode:{self.mode} not supported in MaskedUpsample")

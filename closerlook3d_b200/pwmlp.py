@@ -29,7 +29,7 @@ class _FusedPointWiseMLP(Function):
         ab_pm = ops.sgemm(fa_pm, Cpa, 1, wcat, 1, Cpa, B * N, 2 * Cop, Cpa).view(B, N, 2 * Cop)
         nl.wait()                                   # the search ran on the side stream, overlapping the product
         training = bn.training or (bn.running_mean is None)
-        if any(ctx.needs_input_grad) and training:
+        if any(ctx.needs_input_grad) and (training or ops.deterministic_mode()):
             nl.prefetch_csr(all_slots=True)         # lists for the backward, built behind the forward kernels
         ysel, aq, sq, karg, partial = ops.pwmlp_fwd_stats(ab_pm, wp, sgn, query_xyz, support_xyz, nl.idx, Cout, radius)
         momentum = bn.momentum if bn.momentum is not None else 0.0
@@ -54,12 +54,14 @@ class _FusedPointWiseMLP(Function):
          support_xyz) = ctx.saved_tensors
         B, C, N, M, K, Cout, Cop, Cpa = ctx.dims
         nl = ctx.nl
-        # eval mode (frozen BatchNorm): no batch-statistics terms -> no dense pass, no transposed lists needed
-        off, ent = nl.csr_all_slots() if ctx.training else (None, None)
+        # eval mode (frozen BatchNorm): no batch-statistics terms -> no dense pass, no transposed lists needed, except
+        # in deterministic mode, where every gradient row is gathered over the canonical lists
+        det = ops.deterministic_mode()
+        off, ent = nl.csr_all_slots() if ctx.training or det else (None, None)
         side = pt_utils._side_stream(ysel.device, priority=-1) if pt_utils.overlap_enabled else None
         grad_ab, grad_wp, dgamma, dbeta = ops.pwmlp_bwd(grad_out.contiguous(), bn_bias, ab_pm, wp, sgn, query_xyz, support_xyz, nl.idx,
                                                         off, ent, ysel, aq, sq, karg, stats, bn_weight, ctx.radius,
-                                                        side_stream=side, training=ctx.training)
+                                                        side_stream=side, training=ctx.training, deterministic=det)
         P = B * N
         Cp = ops.padded_channels(C)
         # the two products of the backward are independent: the weight gradient runs on the side stream
@@ -81,7 +83,7 @@ class _FusedPointWiseMLP(Function):
 def forward(module, query_xyz, support_xyz, query_mask, support_mask, support_features):
     conv, bn = module.mlps.conv0[0], module.mlps.conv0[1]
     # a differentiated forward in training mode needs the all-slots transposed lists (BatchNorm2d backward is dense)
-    need_lists = torch.is_grad_enabled() and (bn.training or bn.running_mean is None)
+    need_lists = torch.is_grad_enabled() and (bn.training or bn.running_mean is None or ops.deterministic_mode())
     nl = pt_utils.neighbors(query_xyz, support_xyz, query_mask, support_mask, module.radius, module.nsample,
                             csr="all" if need_lists else None)
     return _FusedPointWiseMLP.apply(support_features.contiguous(), conv.weight, bn.weight, bn.bias, nl, query_xyz,

@@ -110,37 +110,42 @@ int cl3d_nearest_query(const float* query_xyz, const float* support_xyz, const i
  * takes its rank inside its support point's list during the search's emit phase (int atomics), so the list build is
  * a scan plus an atomic-free scatter instead of count + scan + atomic fill.  all_slots = 0: lists over the counted
  * slots k < ncount (avg / sum families); 1: over all K slots (PointWiseMLP: BatchNorm2d sees every slot).
- * csr_off (B,N+1), csr_ent (B,M*K) as cl3d_build_csr.  List order = atomic arrival order (not deterministic).
+ * csr_off (B,N+1), csr_ent (B,M*K) as cl3d_build_csr, with the same list order rule (`deterministic`).
  * phases: 1 = the search (idx / idx_mask / ncount final, ranks left in the workspace), 2 = the lists from those ranks,
  * 3 = both.  A caller that overlaps the list build with the forward kernels issues phase 1, records its "search done"
- * event, then issues phase 2 with the same workspace. */
-size_t cl3d_ball_query_csr_workspace_bytes(int B, int N, int M, int K);
+ * event, then issues phase 2 with the same workspace (and the same `deterministic`). */
+size_t cl3d_ball_query_csr_workspace_bytes(int B, int N, int M, int K, int deterministic);
 int cl3d_ball_query_csr(const float* query_xyz, const float* support_xyz, const int* query_mask,
                         const int* support_mask, int B, int N, int M, float radius, int K, int* idx, int* idx_mask,
                         int* ncount, int all_slots, int* csr_off, int* csr_ent, void* workspace,
-                        size_t workspace_bytes, int algo, int phases, cl3d_stream_t stream);
+                        size_t workspace_bytes, int algo, int phases, int deterministic, cl3d_stream_t stream);
 
 /* Transposed neighbour lists ("who gathers me"), used by the gather-form backward kernels:
  *   csr_off (B,N+1) int32  out: entries of support point j of cloud b are csr_ent[b][off[j]..off[j+1])
  *   csr_ent (B,M*K) int32  out: q*K + k for every counted slot (k < ncount[q]) with idx[q][k] == j
- * workspace: cl3d_csr_workspace_bytes. */
-size_t cl3d_csr_workspace_bytes(int B, int N, int M, int K);
+ * List order: deterministic = 0: atomic arrival order, which varies from run to run.  deterministic = 1: ascending
+ * q*K + k (the order of a serial fill), the same bits on every run; the workspace query takes the same flag (the
+ * canonical pass needs B*M*K + B*N ints more). */
+size_t cl3d_csr_workspace_bytes(int B, int N, int M, int K, int deterministic);
 int cl3d_build_csr(const int* idx, const int* ncount, int B, int N, int M, int K, int* csr_off,
-                   int* csr_ent, void* workspace, size_t workspace_bytes, cl3d_stream_t stream);
+                   int* csr_ent, void* workspace, size_t workspace_bytes, int deterministic, cl3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Compatibility gather / scatter (the reference's materialising path; kept for the non-fused module API).
  * Replace _ext.group_points / _ext.group_points_grad (group_points_gpu.cu:13-33,48-69).
  * ---------------------------------------------------------------------------------------------- */
 /* points / out and grad_out / grad_points in `dtype`.
- * grad_points (B,C,N) is fully overwritten (zero-filled first); contributions are added with fp32 atomics, so the
- * summation order -- like the reference's group_points_grad_gpu.cu:48-69 -- is not deterministic (tolerance parity).
- * A 16-bit gradient is accumulated into `acc` (B*C*N floats of caller scratch; may be NULL for CL3D_DTYPE_F32, which
- * accumulates in grad_points) and converted once. */
+ * grad_points (B,C,N) is fully overwritten.  csr_off / csr_ent NULL: zero-filled first, then contributions are added
+ * with fp32 atomics, so the summation order -- like the reference's group_points_grad_gpu.cu:48-69 -- is not
+ * deterministic (tolerance parity); a 16-bit gradient is accumulated into `acc` (B*C*N floats of caller scratch; may
+ * be NULL for CL3D_DTYPE_F32, which accumulates in grad_points) and converted once.  csr_off / csr_ent given (the
+ * cl3d_build_csr lists of idx over all K slots): each element is the fp32 sum over its list in list order, rounded
+ * once to `dtype`; `acc` is not used.  With canonical lists the result is the same bits on every run. */
 int cl3d_group_points(const void* points /*(B,C,N)*/, int dtype, const int* idx /*(B,M,K)*/, int B, int C, int N,
                       int M, int K, void* out /*(B,C,M,K)*/, cl3d_stream_t stream);
 int cl3d_group_points_grad(const void* grad_out /*(B,C,M,K)*/, int dtype, const int* idx, int B, int C, int N,
-                           int M, int K, void* grad_points, float* acc, cl3d_stream_t stream);
+                           int M, int K, const int* csr_off, const int* csr_ent, void* grad_points, float* acc,
+                           cl3d_stream_t stream);
 
 /* Replaces _ext.masked_grid_subsampling (masked_grid_subsampling_gpu.cu:11-153).
  * sub_xyz (B,m,3) f32, sub_mask (B,m) i32. */
@@ -151,12 +156,15 @@ int cl3d_grid_subsample(const float* points, const int* mask, int B, int n, int 
 
 /* Fused neighbourhood max-pool (body of MaskedMaxPool, pt_utils.py:195-201) and its gradient.
  *   feat_pm (B,N,Cp) point-major (+CL3D_PM_SLACK); out (B,C,M); arg (B,M,Cp) uint8 first arg-max slot (K <= 255)
- *   bwd: grad_pm (B,N,Cp) point-major, zero-filled by the call then accumulated (one red.add row per query).
+ *   bwd: grad_pm (B,N,Cp) point-major.  csr_off / csr_ent NULL: zero-filled by the call then accumulated (one red.add
+ *   row per query; summation order varies from run to run).  Given (the cl3d_build_csr lists of idx over all K
+ *   slots): every row gathered from its list in list order, padded channels 0; canonical lists -> the same bits.
  *   out / grad_out in `dtype` (the maximum of exactly widened values is exact); feat_pm, grad_pm fp32. */
 int cl3d_gather_max_fwd(const float* feat_pm, const int* idx, int B, int N, int M, int K, int C, void* out,
                         int dtype, unsigned char* arg, cl3d_stream_t stream);
 int cl3d_gather_max_bwd(const void* grad_out, int dtype, const int* idx, const unsigned char* arg, int B, int N,
-                        int M, int K, int C, float* grad_pm, cl3d_stream_t stream);
+                        int M, int K, int C, const int* csr_off, const int* csr_ent, float* grad_pm,
+                        cl3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Layout: channel-major (B,C,N) <-> point-major (B,N,Cp), Cp = cl3d_padded_channels(C), pad = 0.
@@ -272,8 +280,12 @@ int cl3d_sgemm_algo(const float* a, long long sa_m, long long sa_k, const float*
  *             two passes, forked from and joined back into `stream` with events (CUDA-graph capturable);
  *             grad_wp (3,Cout) = the -sum da' (x) q/r part of d/dWp (the rest comes out of the weight-gradient
  *             product).  training = 0: BatchNorm2d in eval mode (save_stats = running statistics): its backward
- *             has no batch-statistics terms, dy = sc*dz at the arg-max slot only (csr lists may then be NULL). */
-size_t cl3d_pwmlp_bwd_scratch_floats(int B, int N, int M, int Cout);
+ *             has no batch-statistics terms, dy = sc*dz at the arg-max slot only (csr lists may then be NULL).
+ *             deterministic = 1: no atomics.  The query pass stores d/da' point-major in the scratch, and one
+ *             support-major pass over the (canonical, cl3d_build_csr deterministic = 1) all-slots lists stores every
+ *             grad_ab_pm row once, summed in list order; lists are then required in eval mode too, the side stream
+ *             is not used, and the scratch query takes the same flag (B*M*Cop floats more). */
+size_t cl3d_pwmlp_bwd_scratch_floats(int B, int N, int M, int Cout, int deterministic);
 /* conv weight (Cout, 3+2C) = [Wp|Wc|Wr] + BN gamma -> wcat (2*Cop, Cpa) (rows zero-padded to Cpa), wp (Cout,3),
  * sgn (Cout); and back: d/dwcat (2*Cop, Cpa) + grad_wp (3,Cout) -> d/d(conv weight) (Cout, 3+2C). */
 int cl3d_pwmlp_prep_weights(const float* conv_weight, const float* gamma, int C, int Cout, float* wcat,
@@ -292,8 +304,9 @@ int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta, const flo
                    const float* sgn, const float* query_xyz, const float* support_xyz, const int* idx,
                    const int* csr_off, const int* csr_ent, const float* ysel, const float* aq, const float* sq,
                    const unsigned char* karg, const float* save_stats, const float* gamma, int B, int N,
-                   int M, int K, int Cout, float radius, int training, float* scratch, float* dgamma_dbeta,
-                   float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream, cl3d_stream_t side_stream);
+                   int M, int K, int Cout, float radius, int training, int deterministic, float* scratch,
+                   float* dgamma_dbeta, float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream,
+                   cl3d_stream_t side_stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused multi-shape part-segmentation head (multihead.cu).  Replaces the S per-shape heads of

@@ -44,7 +44,7 @@ def make_ring(dev, B, N, K, n=4):
         d = synth.make_cloud_batch(B, N, 1, 1003 + 7919 * t)
         xyz, mask = d["xyz"].to(dev), d["mask"].to(dev)
         L = _lib.lib()
-        wsb = L.cl3d_ball_query_csr_workspace_bytes(B, N, N, K)
+        wsb = L.cl3d_ball_query_csr_workspace_bytes(B, N, N, K, 0)
         ring.append(dict(xyz=xyz, mask=mask, idx=torch.empty(B, N, K, dtype=torch.int32, device=dev),
                          ncount=torch.empty(B, N, dtype=torch.int32, device=dev),
                          off=torch.empty(B, N + 1, dtype=torch.int32, device=dev),
@@ -59,7 +59,7 @@ def call(b, B, N, K, r, phases):
     p = _lib.ptr
     _lib.check(L.cl3d_ball_query_csr(p(b["xyz"]), p(b["xyz"]), p(b["mask"]), p(b["mask"]), B, N, N, float(r), K,
                                      p(b["idx"]), None, p(b["ncount"]), 0, p(b["off"]), p(b["ent"]), p(b["ws"]),
-                                     b["wsb"], 0, phases, _lib.stream_ptr()), "cl3d_ball_query_csr")
+                                     b["wsb"], 0, phases, 0, _lib.stream_ptr()), "cl3d_ball_query_csr")
 
 
 def timed(fn, ring, launches):

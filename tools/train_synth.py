@@ -6,6 +6,7 @@
         tools/train_synth.py --task scene_segmentation --la pospool_sincos --batch 8 --points 15000
     python tools/train_synth.py --task multi_part_segmentation --dataset shapenetpart --la pseudo_grid
     python tools/train_synth.py --task scene_segmentation --la pseudo_grid --amp bf16
+    python tools/train_synth.py --task classification --deterministic --no-dropout --batch 2 --points 3000 --steps 3 --warmup 0
 
 The reference's training step (function/train_modelnet_dist.py:254-297, train_s3dis_dist.py): forward, loss,
 zero_grad, backward, SGD step, under DistributedDataParallel(broadcast_buffers=False) (:206); part segmentation as function/train_partnet_dist.py:274-282 (multi-shape
@@ -15,6 +16,9 @@ Synthetic data (no datasets in the container): points on noisy unit-sphere shell
 shipped cfgs' radii see realistic neighbour counts), xyz (+1) as input features as the datasets provide them.
 --amp bf16 | fp16 runs forward and loss under torch.autocast (fp16 with a torch.amp.GradScaler); the fused operators
 take the 16-bit features autocast hands them and compute in fp32 inside.
+--deterministic sets CUBLAS_WORKSPACE_CONFIG=:4096:8 before CUDA initialises and turns torch.use_deterministic_algorithms
+on, so two runs from the same state give the same bits; the JSON line then carries every step's loss and a SHA-256 of
+the final parameters and buffers to compare runs by.
 Prints one JSON line: whole-model points/s (device time, max over ranks) and a reference-format checkpoint round trip.
 """
 import argparse
@@ -62,7 +66,13 @@ def main():
                          "gradient buffer + one all-reduce per step (closerlook3d_b200/dist.py)")
     ap.add_argument("--amp", default="off", choices=["off", "bf16", "fp16"],
                     help="mixed precision: forward and loss under torch.autocast in this dtype (fp16 adds a GradScaler)")
+    ap.add_argument("--deterministic", action="store_true",
+                    help="torch.use_deterministic_algorithms(True) with CUBLAS_WORKSPACE_CONFIG=:4096:8: repeatable bits")
+    ap.add_argument("--no-dropout", action="store_true", help="set every Dropout's p to 0")
     args = ap.parse_args()
+    if args.deterministic:
+        os.environ["CUBLAS_WORKSPACE_CONFIG"] = ":4096:8"   # read when cuBLAS initialises: before any CUDA work
+        torch.use_deterministic_algorithms(True)
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     torch.cuda.set_device(local_rank)
@@ -81,9 +91,16 @@ def main():
     build = {"classification": bb.build_classification, "scene_segmentation": bb.build_scene_segmentation,
              "multi_part_segmentation": bb.build_multi_part_segmentation}[args.task]
     torch.manual_seed(0)
+    if args.deterministic:   # the same start: kernel-point dispositions draw from numpy's global generator
+        import numpy as np
+        np.random.seed(0)
     model, criterion = build(cfg)
     model.init_weights()
     model = model.to(device).train()
+    if args.no_dropout:
+        for m in model.modules():
+            if isinstance(m, torch.nn.Dropout):
+                m.p = 0.0
     opt = torch.optim.SGD(model.parameters(), lr=B * world / 16 * 0.002, momentum=0.98, weight_decay=0.001)
     net, flat = model, None
     if world > 1 and args.ddp:
@@ -131,8 +148,9 @@ def main():
             opt.step()
         return loss
 
+    losses = []
     for i in range(args.warmup):
-        step(i)
+        losses.append(step(i).detach())
     pt_utils.cache_stats.update(hit=0, miss=0)
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats(device)
@@ -144,6 +162,7 @@ def main():
     evs[0].record()
     for i in range(args.steps):
         loss = step(args.warmup + i)
+        losses.append(loss.detach())
         evs[i + 1].record()
     torch.cuda.synchronize()
     per = sorted(evs[i].elapsed_time(evs[i + 1]) for i in range(args.steps))
@@ -163,6 +182,11 @@ def main():
         fresh = build(cfg)[0]
         fresh.load_state_dict(ck["model"], strict=True)
         ok = all(torch.equal(a.cpu(), b) for a, b in zip(model.state_dict().values(), fresh.state_dict().values()))
+        import hashlib
+        digest = hashlib.sha256()
+        for k, v in model.state_dict().items():
+            digest.update(k.encode())
+            digest.update(v.detach().cpu().contiguous().reshape(-1).view(torch.uint8).numpy().tobytes())
         print(json.dumps({"what": "whole-model training step (fwd + loss + bwd + SGD), synthetic clouds",
                           "task": args.task, **({"dataset": args.dataset} if part else {}), "local_aggregation": args.la,
                           "amp": args.amp, "n_gpus": world, "clouds_per_gpu": B,
@@ -173,7 +197,9 @@ def main():
                           "points_per_s_median_step": B * N * world / (ms_median * 1e-3), "loss": float(loss.item()),
                           "neighbour_cache_per_step": {k: v / args.steps for k, v in pt_utils.cache_stats.items()},
                           "params_M": sum(p.numel() for p in model.parameters()) / 1e6,
-                          "checkpoint_round_trip": ok, "launch": "eager (no CUDA graph); " + ("DDP broadcast_buffers=False" if args.ddp or world == 1 else
+                          "checkpoint_round_trip": ok, "deterministic": args.deterministic,
+                          "losses": [float(v) for v in torch.stack(losses).float().cpu()],
+                          "state_sha256": digest.hexdigest(), "launch": "eager (no CUDA graph); " + ("DDP broadcast_buffers=False" if args.ddp or world == 1 else
                                                                    "flat gradient buffer, one all-reduce per step")}))
     if world > 1:
         dist.barrier()
