@@ -66,7 +66,7 @@ __device__ __forceinline__ int pg_stage_slots(float4* __restrict__ s_dp, float* 
 
 template <int FAM>
 constexpr int rows_in_flight() {  // independent row loads per lane before they are consumed
-  return (FAM == CL3D_FAM_PSEUDOGRID || FAM == CL3D_FAM_POSPOOL_SINCOS) ? 2 : 4;
+  return FAM == CL3D_FAM_PSEUDOGRID ? 2 : 4;
 }
 template <int FAM, bool BWD>
 constexpr int num_acc() {
@@ -274,12 +274,8 @@ __global__ void __launch_bounds__(kAggWarps * 32, FAM == CL3D_FAM_PSEUDOGRID ? 2
           unsigned roff = 0;
           if (valid) {
             const int j = a.idx[gq * a.K + k0 + lane];
-            dx = __fsub_rn(sxyz[j * 3 + 0], qx), dy = __fsub_rn(sxyz[j * 3 + 1], qy), dz = __fsub_rn(sxyz[j * 3 + 2], qz);
-            if (a.normalize) {  // torch's CUDA `tensor /= python_scalar` multiplies by the fp32 reciprocal
-              dx = __fmul_rn(dx, a.inv_radius);
-              dy = __fmul_rn(dy, a.inv_radius);
-              dz = __fmul_rn(dz, a.inv_radius);
-            }
+            const float3 d = rel_pos(a, sxyz[j * 3 + 0], sxyz[j * 3 + 1], sxyz[j * 3 + 2], qx, qy, qz);
+            dx = d.x, dy = d.y, dz = d.z;
             roff = (unsigned)j * (unsigned)a.Cp;
           }
           if constexpr (FAM == CL3D_FAM_PSEUDOGRID) {
@@ -305,18 +301,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, FAM == CL3D_FAM_PSEUDOGRID ? 2
     for (int i = 0; i < CI; ++i) s_out[(size_t)(lane + 32 * i) * (kTile + 1) + ql] = res[i];
   }
   __syncthreads();
-  // ---- write the tile channel-major + BatchNorm partial moments (one warp per channel row)
-  const int q = q0 + lane;
-  for (int cl = warp; cl < 32 * CI; cl += kAggWarps) {
-    const int c = c0 + cl;
-    if (c >= a.C) break;
-    float v = 0.f;
-    if (q < a.M) {
-      v = s_out[(size_t)cl * (kTile + 1) + lane];
-      a.out[((size_t)b * a.C + c) * a.M + q] = v;
-    }
-    if (a.partial) warp_bn_moments(a.partial, blockIdx.x, a.C, c, v, q < a.M);
-  }
+  store_fwd_tile<true>(a, s_out, 32 * CI, b, q0, [&](int r) { return c0 + r; });
 }
 
 // =================================================================================================
@@ -342,8 +327,6 @@ __global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID ||
   constexpr int NACC = num_acc<FAM, true>();
   constexpr bool PG = FAM == CL3D_FAM_PSEUDOGRID;
   constexpr bool AW = FAM == CL3D_FAM_ADAPTIVE_DP;
-  constexpr bool HASP = AW || PG;
-  constexpr int HS = PG ? kMaxKP : 1;
   const int ppc = params_per_channel<FAM>(a.nkp);
   const SmemLayout L = smem_layout(32 * CI, ppc * 32 * CI);
   float4* s_dp = reinterpret_cast<float4*>(smem + L.dp_off) + (size_t)warp * kSlots;
@@ -404,24 +387,14 @@ __global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID ||
           int rows = min(kSlots, e1 - eb);
           {
             const bool valid = lane < rows;
-            float dx = 0.f, dy = 0.f, dz = 0.f;
-            unsigned roff = 0;
-            int q = 0;
-            if (valid) {
-              q = ent[eb + lane] / a.K;
-              dx = __fsub_rn(px, qxyz[q * 3 + 0]), dy = __fsub_rn(py, qxyz[q * 3 + 1]), dz = __fsub_rn(pz, qxyz[q * 3 + 2]);
-              if (a.normalize) {
-                dx = __fmul_rn(dx, a.inv_radius);
-                dy = __fmul_rn(dy, a.inv_radius);
-                dz = __fmul_rn(dz, a.inv_radius);
-              }
-              roff = (unsigned)q * (unsigned)a.Cp;
-            }
+            BwdEntry e = {0, make_float3(0.f, 0.f, 0.f), 0u};
+            if (valid) e = bwd_entry(a, qxyz, ent[eb + lane], px, py, pz);
             if constexpr (PG) {
-              rows = pg_stage_slots(s_dp, s_h, s_m, valid, dx, dy, dz, roff, a.p0, a.nkp, a.influence, a.inv_extent);
+              rows = pg_stage_slots(s_dp, s_h, s_m, valid, e.dp.x, e.dp.y, e.dp.z, e.roff, a.p0, a.nkp, a.influence,
+                                    a.inv_extent);
             } else if (valid) {
-              s_dp[lane] = make_float4(dx, dy, dz, __uint_as_float(roff));
-              s_h[lane * HS] = a.reduction == CL3D_REDUCE_AVG ? __fdiv_rn(1.f, (float)ncnt[q]) : 1.f;
+              s_dp[lane] = make_float4(e.dp.x, e.dp.y, e.dp.z, __uint_as_float(e.roff));
+              s_h[lane] = a.reduction == CL3D_REDUCE_AVG ? __fdiv_rn(1.f, (float)ncnt[e.q]) : 1.f;
             }
           }
           __syncwarp();
@@ -429,7 +402,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID ||
           __syncwarp();
         }
         // ---- epilogue: gradient w.r.t. this support point's features, parameter gradients
-        if constexpr (HASP) {
+        if constexpr (AW || PG) {
           const float* frow = a.feat_pm + ((size_t)b * a.N + j) * a.Cp + c0 + lane;
 #pragma unroll
           for (int i = 0; i < CI; ++i) {
@@ -458,29 +431,11 @@ __global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID ||
       for (int i = 0; i < CI; ++i) s_out[(size_t)(lane + 32 * i) * (kTile + 1) + jl] = res[i];
     }
     __syncthreads();
-    const int j = j0 + lane;
-    for (int cl = warp; cl < 32 * CI; cl += kAggWarps) {
-      const int c = c0 + cl;
-      if (c >= a.C) break;
-      if (j < a.N) store_out<TO>(s_out[(size_t)cl * (kTile + 1) + lane], a, ((size_t)b * a.C + c) * a.N + j);
-    }
+    store_bwd_tile<TO, true>(a, s_out, 32 * CI, b, j0, [&](int r) { return c0 + r; });
     __syncthreads();
   }
   // ---- CTA-level reduction of the parameter-gradient accumulators, fixed order over the warps
-  if constexpr (AW) {
-    for (int w = 0; w < kAggWarps; ++w) {
-      if (warp == w) {
-#pragma unroll
-        for (int s = 0; s < 4; ++s)
-#pragma unroll
-          for (int i = 0; i < CI; ++i) {
-            float* p = s_red + (size_t)s * 32 * CI + lane + 32 * i;
-            *p = (w == 0) ? pacc[s][i] : (*p + pacc[s][i]);
-          }
-      }
-      __syncthreads();
-    }
-  }
+  if constexpr (AW) aw_bwd_params<CI>(a, pacc, s_red, c0);
   if constexpr (PG) {
     __syncthreads();
     const float* all = s_wk + (size_t)kMaxKP * 32 * CI;  // [warps][kMaxKP][32*CI]
@@ -491,14 +446,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID ||
       s_red[e] = t;
     }
     __syncthreads();
-  }
-  if constexpr (HASP) {
-    // partial layout: (gridDim.x, ppc, C)
-    for (int e = threadIdx.x; e < ppc * 32 * CI; e += blockDim.x) {
-      const int s = e / (32 * CI), cl = e % (32 * CI);
-      const int c = c0 + cl;
-      if (c < a.C) a.partial[((size_t)blockIdx.x * ppc + s) * a.C + c] = s_red[e];
-    }
+    store_param_partial<CI>(a, s_red, ppc, c0);
   }
 }
 
@@ -699,14 +647,8 @@ __global__ void __launch_bounds__(kAggWarps * 32, 3) sincos_fwd_kernel(const Agg
         const int rows = min(kSlots, nrows - k0);
         if (lane < rows) {
           const int j = a.idx[gq * a.K + k0 + lane];
-          float dx = __fsub_rn(sxyz[j * 3 + 0], qx), dy = __fsub_rn(sxyz[j * 3 + 1], qy),
-                dz = __fsub_rn(sxyz[j * 3 + 2], qz);
-          if (a.normalize) {
-            dx = __fmul_rn(dx, a.inv_radius);
-            dy = __fmul_rn(dy, a.inv_radius);
-            dz = __fmul_rn(dz, a.inv_radius);
-          }
-          s_dp[lane] = make_float4(dx, dy, dz, __uint_as_float((unsigned)j * (unsigned)a.Cp));
+          const float3 dp = rel_pos(a, sxyz[j * 3 + 0], sxyz[j * 3 + 1], sxyz[j * 3 + 2], qx, qy, qz);
+          s_dp[lane] = make_float4(dp.x, dp.y, dp.z, __uint_as_float((unsigned)j * (unsigned)a.Cp));
         }
         __syncwarp();
         consume_pairs<PI, false>(feat, s_dp, nullptr, rows, pl, rs, rc);
@@ -727,17 +669,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, 3) sincos_fwd_kernel(const Agg
     }
   }
   __syncthreads();
-  const int q = q0 + lane;
-  for (int r = warp; r < 2 * 32 * PI; r += kAggWarps) {
-    const int c = pair_row_channel(r, p0, 32 * PI, F);
-    if (c < 0) continue;
-    float v = 0.f;
-    if (q < a.M) {
-      v = s_out[(size_t)r * (kTile + 1) + lane];
-      a.out[((size_t)b * a.C + c) * a.M + q] = v;
-    }
-    if (a.partial) warp_bn_moments(a.partial, blockIdx.x, a.C, c, v, q < a.M);
-  }
+  store_fwd_tile<false>(a, s_out, 2 * 32 * PI, b, q0, [&](int r) { return pair_row_channel(r, p0, 32 * PI, F); });
 }
 
 template <int PI, typename TO>
@@ -773,16 +705,9 @@ __global__ void __launch_bounds__(kAggWarps * 32, 3) sincos_bwd_kernel(const Agg
         for (int eb = e0; eb < e1; eb += kSlots) {
           const int rows = min(kSlots, e1 - eb);
           if (lane < rows) {
-            const int q = ent[eb + lane] / a.K;
-            float dx = __fsub_rn(px, qxyz[q * 3 + 0]), dy = __fsub_rn(py, qxyz[q * 3 + 1]),
-                  dz = __fsub_rn(pz, qxyz[q * 3 + 2]);
-            if (a.normalize) {
-              dx = __fmul_rn(dx, a.inv_radius);
-              dy = __fmul_rn(dy, a.inv_radius);
-              dz = __fmul_rn(dz, a.inv_radius);
-            }
-            s_dp[lane] = make_float4(dx, dy, dz, __uint_as_float((unsigned)q * (unsigned)a.Cp));
-            s_h[lane] = a.reduction == CL3D_REDUCE_AVG ? __fdiv_rn(1.f, (float)ncnt[q]) : 1.f;
+            const BwdEntry e = bwd_entry(a, qxyz, ent[eb + lane], px, py, pz);
+            s_dp[lane] = make_float4(e.dp.x, e.dp.y, e.dp.z, __uint_as_float(e.roff));
+            s_h[lane] = a.reduction == CL3D_REDUCE_AVG ? __fdiv_rn(1.f, (float)ncnt[e.q]) : 1.f;
           }
           __syncwarp();
           consume_pairs<PI, true>(gpm, s_dp, s_h, rows, pl, rs, rc);
@@ -796,12 +721,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, 3) sincos_bwd_kernel(const Agg
       }
     }
     __syncthreads();
-    const int j = j0 + lane;
-    for (int r = warp; r < 2 * 32 * PI; r += kAggWarps) {
-      const int c = pair_row_channel(r, p0, 32 * PI, F);
-      if (c < 0) continue;
-      if (j < a.N) store_out<TO>(s_out[(size_t)r * (kTile + 1) + lane], a, ((size_t)b * a.C + c) * a.N + j);
-    }
+    store_bwd_tile<TO, false>(a, s_out, 2 * 32 * PI, b, j0, [&](int r) { return pair_row_channel(r, p0, 32 * PI, F); });
     __syncthreads();
   }
 }
@@ -893,20 +813,18 @@ static int dispatch_sincos(const AggArgs& a, bool bwd, int grid_x, cudaStream_t 
 }
 
 static int dispatch_fwd(int family, int ci, const AggArgs& a, cudaStream_t s) {
-  if (family == CL3D_FAM_POSPOOL_SINCOS) return dispatch_sincos(a, false, a.ntiles, s);
   switch (family) {
     case CL3D_FAM_POSPOOL_XYZ: DISPATCH_CI(launch_fwd, CL3D_FAM_POSPOOL_XYZ, a, s)
-    case CL3D_FAM_POSPOOL_SINCOS: DISPATCH_CI(launch_fwd, CL3D_FAM_POSPOOL_SINCOS, a, s)
+    case CL3D_FAM_POSPOOL_SINCOS: return dispatch_sincos(a, false, a.ntiles, s);
     case CL3D_FAM_ADAPTIVE_DP: DISPATCH_CI(launch_fwd, CL3D_FAM_ADAPTIVE_DP, a, s)
     case CL3D_FAM_PSEUDOGRID: DISPATCH_CI3(launch_fwd, CL3D_FAM_PSEUDOGRID, a, s)
   }
   return CL3D_ERR_UNSUPPORTED;
 }
 static int dispatch_bwd(int family, int ci, const AggArgs& a, int gx, cudaStream_t s) {
-  if (family == CL3D_FAM_POSPOOL_SINCOS) return dispatch_sincos(a, true, gx, s);
   switch (family) {
     case CL3D_FAM_POSPOOL_XYZ: DISPATCH_CI(launch_bwd, CL3D_FAM_POSPOOL_XYZ, a, gx, s)
-    case CL3D_FAM_POSPOOL_SINCOS: DISPATCH_CI(launch_bwd, CL3D_FAM_POSPOOL_SINCOS, a, gx, s)
+    case CL3D_FAM_POSPOOL_SINCOS: return dispatch_sincos(a, true, gx, s);
     case CL3D_FAM_ADAPTIVE_DP: DISPATCH_CI(launch_bwd, CL3D_FAM_ADAPTIVE_DP, a, gx, s)
     case CL3D_FAM_PSEUDOGRID: DISPATCH_CI3(launch_bwd, CL3D_FAM_PSEUDOGRID, a, gx, s)
   }

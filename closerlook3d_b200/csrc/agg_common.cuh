@@ -1,4 +1,5 @@
-// agg_common.cuh -- argument block and tile constants shared by the fused aggregation kernels (agg.cu, pg.cu).
+// agg_common.cuh -- argument block, tile constants and the steps shared by the fused aggregation kernels
+// (agg.cu, agg_max.cu, pg.cu).
 #pragma once
 #include <type_traits>
 
@@ -40,6 +41,90 @@ template <typename TO>
 __device__ __forceinline__ void store_out(float v, const AggArgs& a, size_t i) {
   if constexpr (std::is_same<TO, float>::value) a.out[i] = v;
   else store_f32(reinterpret_cast<TO*>(a.out) + i, v);
+}
+
+// relative position of a neighbour, support - query (pt_utils.py:127-129), divided by the radius when normalising.
+// torch's CUDA `tensor /= python_scalar` multiplies by the fp32 reciprocal; the 1e-5 parity bar depends on rounding
+// exactly as it does.
+__device__ __forceinline__ float3 rel_pos(const AggArgs& a, float sx, float sy, float sz, float qx, float qy, float qz) {
+  float3 d = make_float3(__fsub_rn(sx, qx), __fsub_rn(sy, qy), __fsub_rn(sz, qz));
+  if (a.normalize) {
+    d.x = __fmul_rn(d.x, a.inv_radius);
+    d.y = __fmul_rn(d.y, a.inv_radius);
+    d.z = __fmul_rn(d.z, a.inv_radius);
+  }
+  return d;
+}
+
+// ---------------------------------------------------------------------------------------------
+// one-warp-per-point kernels (agg.cu, agg_max.cu): a CTA handles a tile of kTile centre points, one warp per point,
+// and collects its results in shared memory, s_out[row * (kTile + 1) + point], one row per owned channel.
+// `channel(r)` maps tile row r to its channel.  ORDERED: channels ascend with r, and the first row at or past a.C ends
+// the walk; otherwise a row mapped to a negative channel has none and is skipped.
+// ---------------------------------------------------------------------------------------------
+
+// forward: the tile channel-major into `out` (B,C,M) and each row's BatchNorm moments, one warp per row
+template <bool ORDERED, typename RowChannel>
+__device__ __forceinline__ void store_fwd_tile(const AggArgs& a, const float* s_out, int nrows, int b, int q0,
+                                               RowChannel channel) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int q = q0 + lane;
+  for (int r = warp; r < nrows; r += kAggWarps) {
+    const int c = channel(r);
+    if constexpr (ORDERED) {
+      if (c >= a.C) break;
+    } else if (c < 0) {
+      continue;
+    }
+    float v = 0.f;
+    if (q < a.M) {
+      v = s_out[(size_t)r * (kTile + 1) + lane];
+      a.out[((size_t)b * a.C + c) * a.M + q] = v;
+    }
+    if (a.partial) warp_bn_moments(a.partial, blockIdx.x, a.C, c, v, q < a.M);
+  }
+}
+
+// backward: the tile of d/dfeatures channel-major into `out` (B,C,N)
+template <typename TO, bool ORDERED, typename RowChannel>
+__device__ __forceinline__ void store_bwd_tile(const AggArgs& a, const float* s_out, int nrows, int b, int j0,
+                                               RowChannel channel) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int j = j0 + lane;
+  for (int r = warp; r < nrows; r += kAggWarps) {
+    const int c = channel(r);
+    if constexpr (ORDERED) {
+      if (c >= a.C) break;
+    } else if (c < 0) {
+      continue;
+    }
+    if (j < a.N) store_out<TO>(s_out[(size_t)r * (kTile + 1) + lane], a, ((size_t)b * a.C + c) * a.N + j);
+  }
+}
+
+// backward: one entry en = q * K + slot of a support point's transposed list -- the query q, the relative position
+// of the support point (px, py, pz) to it, and the element offset of q's row in the point-major matrices
+struct BwdEntry {
+  int q;
+  float3 dp;
+  unsigned roff;
+};
+__device__ __forceinline__ BwdEntry bwd_entry(const AggArgs& a, const float* qxyz, int en, float px, float py, float pz) {
+  BwdEntry e;
+  e.q = en / a.K;
+  e.dp = rel_pos(a, px, py, pz, qxyz[e.q * 3 + 0], qxyz[e.q * 3 + 1], qxyz[e.q * 3 + 2]);
+  e.roff = (unsigned)e.q * (unsigned)a.Cp;
+  return e;
+}
+
+// this CTA's rows of the parameter-gradient partials (gridDim.x, ppc, C), from s_red[ppc][32*CI]
+template <int CI>
+__device__ __forceinline__ void store_param_partial(const AggArgs& a, const float* s_red, int ppc, int c0) {
+  for (int e = threadIdx.x; e < ppc * 32 * CI; e += blockDim.x) {
+    const int s = e / (32 * CI), cl = e % (32 * CI);
+    const int c = c0 + cl;
+    if (c < a.C) a.partial[((size_t)blockIdx.x * ppc + s) * a.C + c] = s_red[e];
+  }
 }
 
 
@@ -98,6 +183,26 @@ __device__ __forceinline__ float family_weight(const LaneParams<FAM, CI>& lp, in
   } else {
     return 0.f;
   }
+}
+
+// AdaptiveWeight backward, end of the CTA: sum the warps' accumulators in a fixed order over the warps into
+// s_red[4][32*CI] and write them as this CTA's rows of the (gridDim.x, 4, C) partials
+template <int CI>
+__device__ __forceinline__ void aw_bwd_params(const AggArgs& a, const float (&pacc)[4][CI], float* s_red, int c0) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int w = 0; w < kAggWarps; ++w) {
+    if (warp == w) {
+#pragma unroll
+      for (int s = 0; s < 4; ++s)
+#pragma unroll
+        for (int i = 0; i < CI; ++i) {
+          float* p = s_red + (size_t)s * 32 * CI + lane + 32 * i;
+          *p = (w == 0) ? pacc[s][i] : (*p + pacc[s][i]);
+        }
+    }
+    __syncthreads();
+  }
+  store_param_partial<CI>(a, s_red, 4, c0);
 }
 
 

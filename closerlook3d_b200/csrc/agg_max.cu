@@ -19,7 +19,7 @@ namespace cl3d {
 
 template <int FAM, int CI>
 __global__ void __launch_bounds__(kAggWarps * 32) aggmax_fwd_kernel(const AggArgs a) {
-  __shared__ float s_out[32 * CI][kTile + 1];
+  __shared__ float s_out[32 * CI * (kTile + 1)];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c0 = blockIdx.y * 32 * CI;
   const int tiles_per_cloud = (a.M + kTile - 1) / kTile;
@@ -45,14 +45,10 @@ __global__ void __launch_bounds__(kAggWarps * 32) aggmax_fwd_kernel(const AggArg
         const int rows = min(32, nrows - k0);
         float dx = 0.f, dy = 0.f, dz = 0.f;
         unsigned roff = 0;
-        if (lane < rows) {  // relative position of slot k0+lane (pt_utils.py:127-129)
+        if (lane < rows) {  // relative position of slot k0+lane
           const int j = a.idx[gq * a.K + k0 + lane];
-          dx = __fsub_rn(sxyz[j * 3 + 0], qx), dy = __fsub_rn(sxyz[j * 3 + 1], qy), dz = __fsub_rn(sxyz[j * 3 + 2], qz);
-          if (a.normalize) {
-            dx = __fmul_rn(dx, a.inv_radius);
-            dy = __fmul_rn(dy, a.inv_radius);
-            dz = __fmul_rn(dz, a.inv_radius);
-          }
+          const float3 d = rel_pos(a, sxyz[j * 3 + 0], sxyz[j * 3 + 1], sxyz[j * 3 + 2], qx, qy, qz);
+          dx = d.x, dy = d.y, dz = d.z;
           roff = (unsigned)j * (unsigned)a.Cp;
         }
 #pragma unroll 2
@@ -79,21 +75,10 @@ __global__ void __launch_bounds__(kAggWarps * 32) aggmax_fwd_kernel(const AggArg
         if (c0 + lane + 32 * i < a.Cp) wrow[32 * i] = (unsigned char)win[i];
     }
 #pragma unroll
-    for (int i = 0; i < CI; ++i) s_out[lane + 32 * i][ql] = best[i];
+    for (int i = 0; i < CI; ++i) s_out[(size_t)(lane + 32 * i) * (kTile + 1) + ql] = best[i];
   }
   __syncthreads();
-  // ---- the tile channel-major + BatchNorm partial moments (one warp per channel row), as agg_fwd_kernel
-  const int q = q0 + lane;
-  for (int cl = warp; cl < 32 * CI; cl += kAggWarps) {
-    const int c = c0 + cl;
-    if (c >= a.C) break;
-    float v = 0.f;
-    if (q < a.M) {
-      v = s_out[cl][lane];
-      a.out[((size_t)b * a.C + c) * a.M + q] = v;
-    }
-    if (a.partial) warp_bn_moments(a.partial, blockIdx.x, a.C, c, v, q < a.M);
-  }
+  store_fwd_tile<true>(a, s_out, 32 * CI, b, q0, [&](int r) { return c0 + r; });
 }
 
 template <int FAM, int CI, typename TO>
@@ -101,7 +86,7 @@ __global__ void __launch_bounds__(kAggWarps * 32) aggmax_bwd_kernel(const AggArg
   constexpr bool AW = FAM == CL3D_FAM_ADAPTIVE_DP;
   constexpr int NACC = AW ? 4 : 1;
   __shared__ float s_out[32 * CI][kTile + 1];
-  __shared__ float s_red[NACC][32 * CI];
+  __shared__ float s_red[NACC * 32 * CI];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c0 = blockIdx.y * 32 * CI;
   const int chunkC = min(32 * CI, a.Cp - c0);
@@ -150,12 +135,8 @@ __global__ void __launch_bounds__(kAggWarps * 32) aggmax_bwd_kernel(const AggArg
             const int en = ent[eb + lane];
             const int q = en / a.K;
             slot = en - q * a.K;
-            dx = __fsub_rn(px, qxyz[q * 3 + 0]), dy = __fsub_rn(py, qxyz[q * 3 + 1]), dz = __fsub_rn(pz, qxyz[q * 3 + 2]);
-            if (a.normalize) {
-              dx = __fmul_rn(dx, a.inv_radius);
-              dy = __fmul_rn(dy, a.inv_radius);
-              dz = __fmul_rn(dz, a.inv_radius);
-            }
+            const float3 d = rel_pos(a, px, py, pz, qxyz[q * 3 + 0], qxyz[q * 3 + 1], qxyz[q * 3 + 2]);
+            dx = d.x, dy = d.y, dz = d.z;
             roff = (unsigned)q * (unsigned)a.Cp;
           }
 #pragma unroll 2
@@ -210,24 +191,7 @@ __global__ void __launch_bounds__(kAggWarps * 32) aggmax_bwd_kernel(const AggArg
     }
     __syncthreads();
   }
-  if constexpr (AW) {
-    // CTA-level reduction of the parameter-gradient accumulators in a fixed order over the warps;
-    // partial layout (gridDim.x, 4, C) like agg_bwd_kernel
-    for (int w = 0; w < kAggWarps; ++w) {
-      if (warp == w) {
-#pragma unroll
-        for (int s = 0; s < 4; ++s)
-#pragma unroll
-          for (int i = 0; i < CI; ++i) s_red[s][lane + 32 * i] = (w == 0) ? pacc[s][i] : (s_red[s][lane + 32 * i] + pacc[s][i]);
-      }
-      __syncthreads();
-    }
-    for (int e = threadIdx.x; e < 4 * 32 * CI; e += blockDim.x) {
-      const int s = e / (32 * CI), cl = e % (32 * CI);
-      const int c = c0 + cl;
-      if (c < a.C) a.partial[((size_t)blockIdx.x * 4 + s) * a.C + c] = s_red[s][cl];
-    }
-  }
+  if constexpr (AW) aw_bwd_params<CI>(a, pacc, s_red, c0);
 }
 
 template <int FAM, int CI>

@@ -313,19 +313,11 @@ __global__ void __launch_bounds__(kPgWarps * 32, BWD ? 3 : 4) pg2_kernel(const A
           unsigned roff = 0;
           if (valid) {
             const int r = BWD ? list[eb + lane] / a.K : list[eb + lane];
-            // relative position = support - query in both directions (pt_utils.py:127)
+            // the centre point is the support point in the backward, the query in the forward
             float nx, ny, nz;
             load_xyz(nxyz, r, nx, ny, nz);
-            if constexpr (BWD) {
-              dx = __fsub_rn(cx, nx), dy = __fsub_rn(cy, ny), dz = __fsub_rn(cz, nz);
-            } else {
-              dx = __fsub_rn(nx, cx), dy = __fsub_rn(ny, cy), dz = __fsub_rn(nz, cz);
-            }
-            if (a.normalize) {
-              dx = __fmul_rn(dx, a.inv_radius);
-              dy = __fmul_rn(dy, a.inv_radius);
-              dz = __fmul_rn(dz, a.inv_radius);
-            }
+            const float3 d = BWD ? rel_pos(a, cx, cy, cz, nx, ny, nz) : rel_pos(a, nx, ny, nz, cx, cy, cz);
+            dx = d.x, dy = d.y, dz = d.z;
             roff = (unsigned)r * (unsigned)a.Cp;
           }
           const int n = pg_stage(s_rec, s_ent, valid, dx, dy, dz, roff, s_kx, s_ky, s_kz, a.nkp, a.influence, a.inv_extent,
@@ -682,17 +674,9 @@ __device__ __forceinline__ void pg3_body(const AggArgs& a, int partial_rows) {
         float dx = 0.f, dy = 0.f, dz = 0.f;
         unsigned roff = 0;
         if (valid) {
-          // relative position = support - query in both directions (pt_utils.py:127)
-          if constexpr (BWD) {
-            dx = __fsub_rn(cx, nx), dy = __fsub_rn(cy, ny), dz = __fsub_rn(cz, nz);
-          } else {
-            dx = __fsub_rn(nx, cx), dy = __fsub_rn(ny, cy), dz = __fsub_rn(nz, cz);
-          }
-          if (a.normalize) {
-            dx = __fmul_rn(dx, a.inv_radius);
-            dy = __fmul_rn(dy, a.inv_radius);
-            dz = __fmul_rn(dz, a.inv_radius);
-          }
+          // the centre point is the support point in the backward, the query in the forward
+          const float3 d = BWD ? rel_pos(a, cx, cy, cz, nx, ny, nz) : rel_pos(a, nx, ny, nz, cx, cy, cz);
+          dx = d.x, dy = d.y, dz = d.z;
           roff = (unsigned)r * (unsigned)a.Cp;
         }
         const int n8 = pg3_stage<NT>(h_a, rows_a, rows, valid, dx, dy, dz, roff, s_kx, s_ky, s_kz, a, lane);
