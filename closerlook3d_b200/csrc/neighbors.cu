@@ -35,178 +35,15 @@ __host__ __device__ inline int cell_cap_for(int N) { return N * 4 > 4096 ? N * 4
 // ---------------------------------------------------------------------------------------------
 // grid build
 // ---------------------------------------------------------------------------------------------
-// One CTA per cloud: n_valid = first zero of the mask (the reference stops at the first mask 0,
-// masked_ordered_ball_query_gpu.cu:49-52), bounding box of the valid prefix, grid dimensions.
-__global__ void __launch_bounds__(1024) grid_params_kernel(const float* __restrict__ xyz, const int* __restrict__ mask,
-                                                           int N, float radius, int cell_cap,
-                                                           GridParams* __restrict__ params) {
-  const int b = blockIdx.x;
-  xyz += (size_t)b * N * 3;
-  mask += (size_t)b * N;
-  __shared__ int s_first;
-  __shared__ float s_red[6][32];
-  if (threadIdx.x == 0) s_first = N;
-  __syncthreads();
-  int first = N;
-  for (int i = threadIdx.x; i < N; i += blockDim.x)
-    if (mask[i] == 0) { first = i; break; }
-  if (first < N) atomicMin(&s_first, first);
-  __syncthreads();
-  const int nv = s_first;
-  float mn[3] = {3.0e38f, 3.0e38f, 3.0e38f}, mx[3] = {-3.0e38f, -3.0e38f, -3.0e38f};
-  for (int i = threadIdx.x; i < nv; i += blockDim.x) {
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      float v = xyz[i * 3 + a];
-      mn[a] = fminf(mn[a], v);
-      mx[a] = fmaxf(mx[a], v);
-    }
-  }
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-      mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
-    }
-    if ((threadIdx.x & 31) == 0) {
-      s_red[a][threadIdx.x >> 5] = mn[a];
-      s_red[3 + a][threadIdx.x >> 5] = mx[a];
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const int nw = blockDim.x >> 5;
-    for (int a = 0; a < 3; ++a)
-      for (int w = 1; w < nw; ++w) {
-        s_red[a][0] = fminf(s_red[a][0], s_red[a][w]);
-        s_red[3 + a][0] = fmaxf(s_red[3 + a][0], s_red[3 + a][w]);
-      }
-    GridParams p;
-    p.n_valid = nv;
-    p.pad0 = p.pad1 = p.pad2 = 0;
-    if (nv == 0) {
-      p.ox = p.oy = p.oz = 0.f;
-      p.inv_h = 1.f;
-      p.gx = p.gy = p.gz = 1;
-      p.ncells = 1;
-    } else {
-      float ex = s_red[3][0] - s_red[0][0], ey = s_red[4][0] - s_red[1][0], ez = s_red[5][0] - s_red[2][0];
-      // cell edge strictly larger than the radius: two points closer than `radius` along an axis then land
-      // in the same or adjacent cells even after fp32 rounding of the cell coordinate (< 512 per axis).
-      float h = radius * 1.001f;
-      if (!(h > 1e-20f)) h = 1e-20f;
-      int gx = 1, gy = 1, gz = 1;
-      for (int it = 0; it < 400; ++it) {  // bounded: non-finite coordinates fall back to a single cell
-        float fx = fminf(ex / h, 510.f), fy = fminf(ey / h, 510.f), fz = fminf(ez / h, 510.f);
-        int tx = (int)fx + 1, ty = (int)fy + 1, tz = (int)fz + 1;
-        if ((long long)tx * ty * tz <= (long long)cell_cap && ex / h < 511.f && ey / h < 511.f && ez / h < 511.f) {
-          gx = tx;
-          gy = ty;
-          gz = tz;
-          break;
-        }
-        h *= 1.25f;
-      }
-      p.ox = s_red[0][0];
-      p.oy = s_red[1][0];
-      p.oz = s_red[2][0];
-      p.inv_h = 1.0f / h;
-      p.gx = gx;
-      p.gy = gy;
-      p.gz = gz;
-      p.ncells = gx * gy * gz;
-    }
-    params[b] = p;
-  }
-}
-
 __device__ __forceinline__ int cell_coord(float x, float o, float inv_h, int g) {
   int c = (int)((x - o) * inv_h);
   return c < 0 ? 0 : (c >= g ? g - 1 : c);
 }
 
-__global__ void zero_cells_kernel(const GridParams* __restrict__ params, int cell_cap, int* __restrict__ cell_cnt) {
-  const int b = blockIdx.y;
-  const int nc = params[b].ncells;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nc; i += gridDim.x * blockDim.x)
-    cell_cnt[(size_t)b * cell_cap + i] = 0;
-}
-
-// cell id + arrival rank inside the cell (one int atomic per point)
-__global__ void cell_count_kernel(const float* __restrict__ xyz, const GridParams* __restrict__ params, int N,
-                                  int cell_cap, int* __restrict__ cell_cnt, int2* __restrict__ cell_rank) {
-  const int b = blockIdx.y;
-  const GridParams p = params[b];
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= p.n_valid) return;
-  const float* q = xyz + ((size_t)b * N + i) * 3;
-  int cx = cell_coord(q[0], p.ox, p.inv_h, p.gx);
-  int cy = cell_coord(q[1], p.oy, p.inv_h, p.gy);
-  int cz = cell_coord(q[2], p.oz, p.inv_h, p.gz);
-  int cell = cx + p.gx * (cy + p.gy * cz);
-  int r = atomicAdd(&cell_cnt[(size_t)b * cell_cap + cell], 1);
-  cell_rank[(size_t)b * N + i] = make_int2(cell, r);
-}
-
-// exclusive scan of the per-cell counts of one cloud (one CTA per cloud)
-__global__ void __launch_bounds__(1024) cell_scan_kernel(const GridParams* __restrict__ params, int cell_cap,
-                                                         const int* __restrict__ cell_cnt,
-                                                         int* __restrict__ cell_start) {
-  const int b = blockIdx.x;
-  const int nc = params[b].ncells;
-  cell_cnt += (size_t)b * cell_cap;
-  cell_start += (size_t)b * (cell_cap + 1);
-  __shared__ int s_warp[32];
-  const int per = (nc + blockDim.x - 1) / blockDim.x;
-  const int lo = min((int)threadIdx.x * per, nc), hi = min(lo + per, nc);
-  int sum = 0;
-  for (int i = lo; i < hi; ++i) sum += cell_cnt[i];
-  // block exclusive scan of `sum`
-  int v = sum;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) >= o) v += t;
-  }
-  if ((threadIdx.x & 31) == 31) s_warp[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    int w = threadIdx.x < (blockDim.x >> 5) ? s_warp[threadIdx.x] : 0;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, w, o);
-      if (threadIdx.x >= o) w += t;
-    }
-    s_warp[threadIdx.x] = w;
-  }
-  __syncthreads();
-  int base = v - sum + ((threadIdx.x >> 5) > 0 ? s_warp[(threadIdx.x >> 5) - 1] : 0);
-  for (int i = lo; i < hi; ++i) {
-    cell_start[i] = base;
-    base += cell_cnt[i];
-  }
-  if (threadIdx.x == blockDim.x - 1) cell_start[nc] = base;  // last thread's running total == n_valid
-}
-
-__global__ void cell_fill_kernel(const float* __restrict__ xyz, const GridParams* __restrict__ params, int N,
-                                 int cell_cap, const int* __restrict__ cell_start,
-                                 const int2* __restrict__ cell_rank, float4* __restrict__ sorted) {
-  const int b = blockIdx.y;
-  const int nv = params[b].n_valid;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= nv) return;
-  const float* q = xyz + ((size_t)b * N + i) * 3;
-  int2 cr = cell_rank[(size_t)b * N + i];
-  int pos = cell_start[(size_t)b * (cell_cap + 1) + cr.x] + cr.y;
-  sorted[(size_t)b * N + pos] = make_float4(q[0], q[1], q[2], __int_as_float(i));
-}
-
-// Whole grid build of one cloud in ONE kernel (one CTA of 1024 threads per cloud) when the cell counters fit in
-// shared memory: valid prefix + bounding box + grid dimensions, cell counts with shared-memory atomics, exclusive scan,
-// scatter into cell order.  The BASELINE clouds have 10^3 .. 15^3 cells, so this replaces the five dependent launches
-// (params, zero, count, scan, fill: ~40 us of mostly launch latency at c3, r1n launch list) on the search's critical
-// path.  Larger grids use the same kernel with the counters in global memory.
+// The whole grid build of a cloud is one CTA of 1024 threads: valid prefix (the reference stops at the first mask 0,
+// masked_ordered_ball_query_gpu.cu:49-52), bounding box, grid dimensions, cell counts, exclusive scan, scatter into
+// cell order.  The cell counters live in shared memory up to kFusedGridCells cells (every BASELINE cloud: 10^3 .. 15^3
+// cells), so counting is shared-memory atomics; larger grids keep them in the cloud's slice of the workspace.
 constexpr int kFusedGridCells = 12288;   // 48 KB of counters
 
 __device__ __forceinline__ GridParams make_grid_params(int nv, const float (&mn)[3], const float (&mx)[3], float radius,
@@ -247,6 +84,30 @@ __device__ __forceinline__ GridParams make_grid_params(int nv, const float (&mn)
   p.gz = gz;
   p.ncells = gx * gy * gz;
   return p;
+}
+
+// Block-wide exclusive scan of one value per thread: returns the sum of the values of the threads before this one.
+// Warp scan, then a scan of the warps' totals in s_warp[32].  Every thread of the block calls it.
+__device__ __forceinline__ int block_exclusive_scan(int sum, int* s_warp) {
+  int v = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) >= o) v += t;
+  }
+  if ((threadIdx.x & 31) == 31) s_warp[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    int w = threadIdx.x < (blockDim.x >> 5) ? s_warp[threadIdx.x] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, w, o);
+      if (threadIdx.x >= o) w += t;
+    }
+    s_warp[threadIdx.x] = w;
+  }
+  __syncthreads();
+  return v - sum + ((threadIdx.x >> 5) > 0 ? s_warp[(threadIdx.x >> 5) - 1] : 0);
 }
 
 __global__ void __launch_bounds__(1024) grid_build_fused_kernel(const float* __restrict__ xyz, const int* __restrict__ mask,
@@ -375,25 +236,7 @@ __global__ void __launch_bounds__(1024) grid_build_fused_kernel(const float* __r
   const int lo = min((int)threadIdx.x * per, p.ncells), hi = min(lo + per, p.ncells);
   int sum = 0;
   for (int c = lo; c < hi; ++c) sum += s_cnt[c];
-  int v = sum;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) >= o) v += t;
-  }
-  if ((threadIdx.x & 31) == 31) s_warp[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    int w = threadIdx.x < (blockDim.x >> 5) ? s_warp[threadIdx.x] : 0;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, w, o);
-      if (threadIdx.x >= o) w += t;
-    }
-    s_warp[threadIdx.x] = w;
-  }
-  __syncthreads();
-  int base = v - sum + ((threadIdx.x >> 5) > 0 ? s_warp[(threadIdx.x >> 5) - 1] : 0);
+  int base = block_exclusive_scan(sum, s_warp);
   for (int c = lo; c < hi; ++c) {
     const int n = s_cnt[c];
     s_cnt[c] = base;
@@ -424,6 +267,45 @@ __global__ void __launch_bounds__(1024) grid_build_fused_kernel(const float* __r
                                                __int_as_float(i));
     }
   }
+}
+
+// The grid's workspace, one slice per cloud in each region.  grid_workspace(nullptr, ...) only sizes it.
+struct GridWorkspace {
+  int cap;               // cells per cloud at most
+  GridParams* params;    // B
+  int* cell_cnt;         // B x cap: the counters of grids above kFusedGridCells cells
+  int* cell_start;       // B x (cap + 1)
+  int2* cell_rank;       // B x N: cell id + arrival rank in the cell
+  float4* sorted;        // B x N: {x, y, z, index} in cell order
+  size_t bytes;
+};
+
+static GridWorkspace grid_workspace(void* base, int B, int N) {
+  GridWorkspace g;
+  g.cap = cell_cap_for(N);
+  size_t off = 0;
+  auto take = [&](size_t n) {
+    void* p = base ? (unsigned char*)base + off : nullptr;
+    off += align_up(n, 256);
+    return p;
+  };
+  g.params = (GridParams*)take(sizeof(GridParams) * (size_t)B);
+  g.cell_cnt = (int*)take(sizeof(int) * (size_t)B * g.cap);
+  g.cell_start = (int*)take(sizeof(int) * (size_t)B * (g.cap + 1));
+  g.cell_rank = (int2*)take(sizeof(int2) * (size_t)B * N);
+  g.sorted = (float4*)take(sizeof(float4) * (size_t)B * N);
+  g.bytes = off;
+  return g;
+}
+
+// every cloud's valid supports into its cell grid, one CTA per cloud
+static void build_grid(const float* support_xyz, const int* support_mask, int B, int N, float radius,
+                       const GridWorkspace& g, cudaStream_t stream) {
+  static std::atomic<unsigned long long> attr{0};
+  allow_big_smem(grid_build_fused_kernel, attr);
+  grid_build_fused_kernel<<<B, 1024, kFusedGridCells * sizeof(int), stream>>>(support_xyz, support_mask, N, radius,
+                                                                              g.cap, g.params, g.cell_cnt, g.cell_start,
+                                                                              g.cell_rank, g.sorted); CL3D_LAUNCHED(1);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -918,25 +800,7 @@ __global__ void __launch_bounds__(1024) csr_scan_kernel(int N, const int* __rest
   const int lo = min(threadIdx.x * per, N), hi = min(lo + per, N);
   int sum = 0;
   for (int i = lo; i < hi; ++i) sum += cnt[i];
-  int v = sum;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) >= o) v += t;
-  }
-  if ((threadIdx.x & 31) == 31) s_warp[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    int w = threadIdx.x < (blockDim.x >> 5) ? s_warp[threadIdx.x] : 0;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, w, o);
-      if (threadIdx.x >= o) w += t;
-    }
-    s_warp[threadIdx.x] = w;
-  }
-  __syncthreads();
-  int base = v - sum + ((threadIdx.x >> 5) > 0 ? s_warp[(threadIdx.x >> 5) - 1] : 0);
+  int base = block_exclusive_scan(sum, s_warp);
   for (int i = lo; i < hi; ++i) {
     off[i] = base;
     if (cursor) cursor[i] = base;
@@ -1092,14 +956,7 @@ extern "C" size_t cl3d_ball_query_workspace_bytes(int B, int N, int M, int K) {
   (void)M;
   (void)K;
   if (B <= 0 || N <= 0) return 256;
-  const size_t cap = (size_t)cell_cap_for(N);
-  size_t s = 0;
-  s += align_up(sizeof(GridParams) * (size_t)B, 256);
-  s += align_up(sizeof(int) * (size_t)B * cap, 256);        // cell_cnt
-  s += align_up(sizeof(int) * (size_t)B * (cap + 1), 256);  // cell_start
-  s += align_up(sizeof(int2) * (size_t)B * N, 256);         // cell id + rank
-  s += align_up(sizeof(float4) * (size_t)B * N, 256);       // cell-sorted points
-  return s;
+  return grid_workspace(nullptr, B, N).bytes;
 }
 
 static int ball_query_impl(const float* query_xyz, const float* support_xyz, const int* query_mask,
@@ -1189,32 +1046,8 @@ static int ball_query_impl(const float* query_xyz, const float* support_xyz, con
               cl3d_ball_query_workspace_bytes(B, N, M, K));
     return CL3D_ERR_WORKSPACE;
   }
-  const int cap = cell_cap_for(N);
-  unsigned char* w = (unsigned char*)workspace;
-  GridParams* params = (GridParams*)w;
-  w += align_up(sizeof(GridParams) * (size_t)B, 256);
-  int* cell_cnt = (int*)w;
-  w += align_up(sizeof(int) * (size_t)B * cap, 256);
-  int* cell_start = (int*)w;
-  w += align_up(sizeof(int) * (size_t)B * (cap + 1), 256);
-  int2* cell_rank = (int2*)w;
-  w += align_up(sizeof(int2) * (size_t)B * N, 256);
-  float4* sorted = (float4*)w;
-
-  if (getenv("CL3D_GRID_BUILD_V1")) {  // A/B switch: the five-kernel build
-    grid_params_kernel<<<B, 1024, 0, stream>>>(support_xyz, support_mask, N, radius, cap, params); CL3D_LAUNCHED(1);
-    zero_cells_kernel<<<dim3(64, B), 256, 0, stream>>>(params, cap, cell_cnt); CL3D_LAUNCHED(1);
-    cell_count_kernel<<<dim3(ceil_div(N, 256), B), 256, 0, stream>>>(support_xyz, params, N, cap, cell_cnt, cell_rank); CL3D_LAUNCHED(1);
-    cell_scan_kernel<<<B, 1024, 0, stream>>>(params, cap, cell_cnt, cell_start); CL3D_LAUNCHED(1);
-    cell_fill_kernel<<<dim3(ceil_div(N, 256), B), 256, 0, stream>>>(support_xyz, params, N, cap, cell_start, cell_rank,
-                                                                    sorted); CL3D_LAUNCHED(1);
-  } else {
-    static std::atomic<unsigned long long> attr_build{0};
-    allow_big_smem(grid_build_fused_kernel, attr_build);
-    grid_build_fused_kernel<<<B, 1024, kFusedGridCells * sizeof(int), stream>>>(support_xyz, support_mask, N, radius, cap,
-                                                                                params, cell_cnt, cell_start, cell_rank,
-                                                                                sorted); CL3D_LAUNCHED(1);
-  }
+  const GridWorkspace g = grid_workspace(workspace, B, N);
+  build_grid(support_xyz, support_mask, B, N, radius, g, stream);
   size_t smem = (size_t)kBQWarps * (kCandCap + cap3k) * 8 + (size_t)kBQWarps * K * 4;
   static std::atomic<unsigned long long> attr_grid{0};
   if (first_call_on_device(attr_grid))
@@ -1223,7 +1056,7 @@ static int ball_query_impl(const float* query_xyz, const float* support_xyz, con
   // the same points and mask as query and support (every non-strided layer): walk the queries in cell order
   const int cell_order = query_xyz == support_xyz && query_mask == support_mask && M == N;
   ball_query_grid_kernel<<<(unsigned)((total + kBQWarps - 1) / kBQWarps), kBQWarps * 32, smem, stream>>>(
-      query_xyz, support_xyz, query_mask, params, cell_start, sorted, B, N, M, radius, K, cap, cell_order, idx,
+      query_xyz, support_xyz, query_mask, g.params, g.cell_start, g.sorted, B, N, M, radius, K, g.cap, cell_order, idx,
       idx_mask, ncount, csr_cnt, csr_rank, csr_all); CL3D_LAUNCHED(1);
   return check_launch("ball_query_grid_kernel");
 }
@@ -1252,25 +1085,11 @@ extern "C" int cl3d_nearest_query(const float* query_xyz, const float* support_x
               cl3d_nearest_query_workspace_bytes(B, N, M));
     return CL3D_ERR_WORKSPACE;
   }
-  const int cap = cell_cap_for(N);
-  unsigned char* w = (unsigned char*)workspace;
-  GridParams* params = (GridParams*)w;
-  w += align_up(sizeof(GridParams) * (size_t)B, 256);
-  int* cell_cnt = (int*)w;
-  w += align_up(sizeof(int) * (size_t)B * cap, 256);
-  int* cell_start = (int*)w;
-  w += align_up(sizeof(int) * (size_t)B * (cap + 1), 256);
-  int2* cell_rank = (int2*)w;
-  w += align_up(sizeof(int2) * (size_t)B * N, 256);
-  float4* sorted = (float4*)w;
   // no radius here: the build picks the smallest cell edge whose grid fits the cell budget (4 cells per point)
-  static std::atomic<unsigned long long> attr_build{0};
-  allow_big_smem(grid_build_fused_kernel, attr_build);
-  grid_build_fused_kernel<<<B, 1024, kFusedGridCells * sizeof(int), stream>>>(support_xyz, support_mask, N, 0.f, cap,
-                                                                              params, cell_cnt, cell_start, cell_rank,
-                                                                              sorted); CL3D_LAUNCHED(1);
-  nearest_query_grid_kernel<<<dim3(ceil_div(M, 256), B), 256, 0, stream>>>(query_xyz, query_mask, params, cell_start,
-                                                                           sorted, N, M, cap, idx, idx_mask); CL3D_LAUNCHED(1);
+  const GridWorkspace g = grid_workspace(workspace, B, N);
+  build_grid(support_xyz, support_mask, B, N, 0.f, g, stream);
+  nearest_query_grid_kernel<<<dim3(ceil_div(M, 256), B), 256, 0, stream>>>(query_xyz, query_mask, g.params, g.cell_start,
+                                                                           g.sorted, N, M, g.cap, idx, idx_mask); CL3D_LAUNCHED(1);
   return check_launch("nearest_query_grid_kernel");
 }
 

@@ -45,25 +45,10 @@ class _FusedAggBNReLU(Function):
         arg = None
         if spec.reduction == ops.REDUCE["max"]:   # winning slot per (query, channel), read again by the backward
             arg = torch.empty(B, M, feat_pm.shape[2], dtype=torch.uint8, device=features.device)
-        if nl.parts:
-            assert arg is None, "batch-parts search is an experiment for the sum / avg reductions"
-            # the batch was searched in parts: aggregate part h as soon as ITS search is done, beside the search of h+1
-            L = ops._lib.lib()
-            agg = torch.empty(B, C, M, dtype=torch.float32, device=features.device)
-            tpc = L.cl3d_agg_num_tiles(1, M)      # BatchNorm partial rows per cloud
-            partial = ops.bn_partial_buffer(B * tpc, C, features.device) if training else None
-            cur = torch.cuda.current_stream()
-            for b0, b1, ev in nl.parts:
-                cur.wait_event(ev)
-                ops.agg_fwd(spec.family, spec.reduction, feat_pm[b0:b1], query_xyz[b0:b1], support_xyz[b0:b1],
-                            nl.idx[b0:b1], nl.ncount[b0:b1], p0, p1, C, spec.radius, spec.normalize, spec.shared,
-                            spec.nkp, spec.extent, spec.influence, want_bn_partial=training,
-                            out=(agg[b0:b1], partial[b0 * tpc:b1 * tpc] if training else None))
-        else:
-            nl.wait()
-            agg, partial = ops.agg_fwd(spec.family, spec.reduction, feat_pm, query_xyz, support_xyz, nl.idx, nl.ncount,
-                                       p0, p1, C, spec.radius, spec.normalize, spec.shared, spec.nkp, spec.extent,
-                                       spec.influence, want_bn_partial=training, arg=arg)
+        nl.wait()
+        agg, partial = ops.agg_fwd(spec.family, spec.reduction, feat_pm, query_xyz, support_xyz, nl.idx, nl.ncount,
+                                   p0, p1, C, spec.radius, spec.normalize, spec.shared, spec.nkp, spec.extent,
+                                   spec.influence, want_bn_partial=training, arg=arg)
         momentum = bn.momentum if bn.momentum is not None else 0.0
         if training and bn.running_mean is not None:
             bn.num_batches_tracked.add_(1)

@@ -81,14 +81,13 @@ def _empty_pm(B, N, W, device):
 
 @_on_device
 def ball_query(query_xyz, support_xyz, query_mask, support_mask, radius, nsample, want_mask=True, want_ncount=True,
-               algo=0, csr=None, after_search=None, out=None, deterministic=None):
+               algo=0, csr=None, after_search=None, deterministic=None):
     """-> (idx (B,M,K) i32, idx_mask (B,M,K) i32 | None, ncount (B,M) i32 | None); bit-exact with the
     reference's masked_ordered_ball_query (masked_ordered_ball_query_gpu.cu:11-96).
     csr = "counted" | "all": also build the transposed lists in the same call (cl3d_ball_query_csr) and return
     (idx, idx_mask, ncount, (csr_off, csr_ent)).  after_search(): called between the search and the list build (the
     caller records its "search done" event there, so consumers of idx do not wait for the lists).
-    out: dict of preallocated result tensors (idx, idx_mask, ncount, off, ent -- e.g. batch slices of larger tensors)
-    to write into instead of allocating.  deterministic (None: torch's flag): the lists in canonical order."""
+    deterministic (None: torch's flag): the lists in canonical order."""
     require_cuda(query_xyz, "query_xyz", F32)
     require_cuda(support_xyz, "support_xyz", F32)
     require_cuda(query_mask, "query_mask", I32)
@@ -98,15 +97,13 @@ def ball_query(query_xyz, support_xyz, query_mask, support_mask, radius, nsample
     K = int(nsample)
     dev = query_xyz.device
     L = _lib.lib()
-    out = out or {}
-    idx = out["idx"] if "idx" in out else torch.empty(B, M, K, dtype=I32, device=dev)
-    idx_mask = out.get("idx_mask") if "idx" in out else (torch.empty(B, M, K, dtype=I32, device=dev) if want_mask else None)
-    ncount = out["ncount"] if "ncount" in out else \
-        (torch.empty(B, M, dtype=I32, device=dev) if (want_ncount or csr) else None)
+    idx = torch.empty(B, M, K, dtype=I32, device=dev)
+    idx_mask = torch.empty(B, M, K, dtype=I32, device=dev) if want_mask else None
+    ncount = torch.empty(B, M, dtype=I32, device=dev) if (want_ncount or csr) else None
     if csr:
         assert csr in ("counted", "all")
-        off = out["off"] if "off" in out else torch.empty(B, N + 1, dtype=I32, device=dev)
-        ent = out["ent"] if "ent" in out else torch.empty(B, M * K, dtype=I32, device=dev)
+        off = torch.empty(B, N + 1, dtype=I32, device=dev)
+        ent = torch.empty(B, M * K, dtype=I32, device=dev)
         det = int(deterministic_mode(deterministic))
         wsb = L.cl3d_ball_query_csr_workspace_bytes(B, N, M, K, det)
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
@@ -248,18 +245,15 @@ def bn_partial_moments(partial):
 
 @_on_device
 def agg_fwd(family, reduction, feat_pm, query_xyz, support_xyz, idx, ncount, p0, p1, C, radius, normalize, shared=1,
-            nkp=0, extent=1.0, influence=0, want_bn_partial=True, out=None, arg=None):
-    """-> (agg (B,C,M), bn_partial (ntiles,BN_PARTIAL_ROWS,C) | None); out = (agg, partial) preallocated (e.g. batch slices);
+            nkp=0, extent=1.0, influence=0, want_bn_partial=True, arg=None):
+    """-> (agg (B,C,M), bn_partial (ntiles,BN_PARTIAL_ROWS,C) | None);
     arg = (B,M,Cp) uint8 buffer for the winning slots, required by (and only by) the max reduction"""
     B, N, Cp = feat_pm.shape
     M, K = idx.shape[1], idx.shape[2]
     L = _lib.lib()
     dev = feat_pm.device
-    if out is not None:
-        agg, partial = out
-    else:
-        agg = torch.empty(B, C, M, dtype=F32, device=dev)
-        partial = bn_partial_buffer(L.cl3d_agg_num_tiles(B, M), C, dev) if want_bn_partial else None
+    agg = torch.empty(B, C, M, dtype=F32, device=dev)
+    partial = bn_partial_buffer(L.cl3d_agg_num_tiles(B, M), C, dev) if want_bn_partial else None
     check(L.cl3d_agg_fwd(family, reduction, ptr(feat_pm), ptr(query_xyz), ptr(support_xyz), ptr(idx), ptr(ncount),
                          ptr(p0), ptr(p1), B, N, M, K, C, float(radius), int(normalize), int(shared), int(nkp),
                          float(extent), int(influence), ptr(agg), ptr(partial), ptr(arg), stream_ptr()), "cl3d_agg_fwd")

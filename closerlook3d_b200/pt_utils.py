@@ -43,7 +43,6 @@ class NeighborList:
         self._csr = None
         self._csr_all = None
         self._csr_det = self._csr_all_det = False   # whether each list set is canonical (ops.deterministic_mode)
-        self.parts = None          # [(b0, b1, search-done event)] when the batch was searched in parts
         self.event = None
         self._csr_event = None
         self._csr_all_event = None
@@ -113,10 +112,6 @@ class NeighborList:
 
 _SIDE = {}
 overlap_enabled = True  # run the neighbour search on a side stream (fork/join), see NeighborList
-# Search the clouds of a batch in this many parts (clouds are independent).  The fused operators start the forward of
-# part 0 as soon as ITS search is done, so the issue-bound search of part 1 runs beside the L1-bound aggregation of
-# part 0 instead of in front of it.  1 = off.
-batch_parts = 1   # splitting the batch trades overlap of search and aggregation for half-batch kernels with larger tail effects
 
 
 def _side_stream(device, priority=0):
@@ -167,44 +162,21 @@ def neighbors(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
         cur = torch.cuda.current_stream()
         side = _side_stream(query_xyz.device)
         side.wait_stream(cur)
-        B = query_xyz.shape[0]
-        nparts = max(1, min(int(batch_parts), B)) if csr else 1   # parts only pay off when a fused forward follows
-        parts = None
         with torch.cuda.stream(side):
-            if nparts == 1:
-                ev = torch.cuda.Event()      # search done: idx / ncount final (the forward kernels wait for this one)
-                res = ops.ball_query(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
-                                     want_mask=need_mask, want_ncount=True, csr=csr,
-                                     after_search=(lambda: ev.record(side)) if csr else None, deterministic=det)
-                if not csr:
-                    ev.record(side)
-                idx, idx_mask, ncount = res[:3]
-                lists = res[3] if csr else None
-            else:
-                M, N, K, dev = query_xyz.shape[1], support_xyz.shape[1], int(nsample), query_xyz.device
-                idx = torch.empty(B, M, K, dtype=torch.int32, device=dev)
-                idx_mask = torch.empty(B, M, K, dtype=torch.int32, device=dev) if need_mask else None
-                ncount = torch.empty(B, M, dtype=torch.int32, device=dev)
-                lists = (torch.empty(B, N + 1, dtype=torch.int32, device=dev),
-                         torch.empty(B, M * K, dtype=torch.int32, device=dev))
-                parts = []
-                for h in range(nparts):
-                    b0, b1 = (B * h) // nparts, (B * (h + 1)) // nparts
-                    evh = torch.cuda.Event()
-                    out = dict(idx=idx[b0:b1], idx_mask=idx_mask[b0:b1] if need_mask else None, ncount=ncount[b0:b1],
-                               off=lists[0][b0:b1], ent=lists[1][b0:b1])
-                    ops.ball_query(query_xyz[b0:b1], support_xyz[b0:b1], query_mask[b0:b1], support_mask[b0:b1], radius,
-                                   nsample, want_mask=need_mask, want_ncount=True, csr=csr, out=out,
-                                   after_search=(lambda e=evh: e.record(side)), deterministic=det)
-                    parts.append((b0, b1, evh))
-                ev = parts[-1][2]            # every part searched (stream order)
+            ev = torch.cuda.Event()          # search done: idx / ncount final (the forward kernels wait for this one)
+            res = ops.ball_query(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
+                                 want_mask=need_mask, want_ncount=True, csr=csr,
+                                 after_search=(lambda: ev.record(side)) if csr else None, deterministic=det)
+            if not csr:
+                ev.record(side)
+            idx, idx_mask, ncount = res[:3]
+            lists = res[3] if csr else None
             ev_lists = None
             if csr:                          # lists done: only the backward waits for this one
                 ev_lists = torch.cuda.Event()
                 ev_lists.record(side)
         nl = NeighborList(idx, ncount, idx_mask, support_xyz.shape[1])
         nl.event = ev
-        nl.parts = parts
     else:
         res = ops.ball_query(query_xyz, support_xyz, query_mask, support_mask, radius, nsample,
                              want_mask=need_mask, want_ncount=True, csr=csr, deterministic=det)

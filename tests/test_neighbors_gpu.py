@@ -49,6 +49,7 @@ CASES = [
     (1, 5, 5, 4, 0.5, "cube", 0),                  # tiny
     (1, 5, 5, 4, 0.5, "cube", 2),
     (2, 3000, 3000, 40, 0.02, "cube", 2),          # almost empty balls: cnt < K, cyclic padding
+    (2, 15000, 15000, 16, 0.03, "cube", 2),        # 34^3 = 39304 cells > kFusedGridCells: cell counters in global memory
     (8, 15000, 15000, 26, None, "cube", 0),        # BASELINE c3 shape
 ]
 

@@ -7,8 +7,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from closerlook3d_b200.config import baseline_config
 
 MAP = [("gemm_tf32x3", "cl3d_sgemm_algo"), ("sgemm", "cl3d_sgemm_algo"), ("splitk_reduce", "cl3d_sgemm_algo"),
-       ("ball_query", "cl3d_ball_query_csr"), ("grid_build_fused", "cl3d_ball_query_csr"), ("grid_params", "cl3d_ball_query_csr"),
-       ("cell_", "cl3d_ball_query_csr"), ("zero_cells", "cl3d_ball_query_csr"), ("csr_", "cl3d_ball_query_csr"),
+       ("ball_query", "cl3d_ball_query_csr"), ("grid_build_fused", "cl3d_ball_query_csr"), ("csr_", "cl3d_ball_query_csr"),
        ("pg2_kernel<(bool)0", "cl3d_agg_fwd"), ("pg2_kernel<(bool)1", "cl3d_agg_bwd"), ("pg2_kernel<0", "cl3d_agg_fwd"),
        ("pg2_kernel<1", "cl3d_agg_bwd"), ("pg3_bwd_kernel", "cl3d_agg_bwd"), ("aggmax_fwd", "cl3d_agg_fwd"),
        ("aggmax_bwd", "cl3d_agg_bwd"), ("nearest_query", "cl3d_nearest_query"),
