@@ -1,11 +1,10 @@
 // agg.cu -- fused local aggregation, forward and backward, for the per-(channel, neighbour)-weight families
-//           PosPool(xyz | sin_cos), AdaptiveWeight(dp) and PseudoGrid (sm_90a).
+//           PosPool(xyz | sin_cos) and AdaptiveWeight(dp) (sm_90a).
 //
 // Replaces, per LocalAggregation call of the reference
 //   /root/reference/pytorch/ops/pt_custom_ops/pt_utils.py:121-144            (2x group_points, subtract, normalise)
 //   /root/reference/pytorch/models/local_aggregation_operators.py:65-105      (PosPool transform + reduction)
 //   .../local_aggregation_operators.py:188-217                                (AdaptiveWeight)
-//   .../local_aggregation_operators.py:384-419                                (PseudoGrid)
 // none of which exists as a fused kernel there: the reference materialises (B,C,M,K) tensors ~10 times.
 //
 // Forward  (one warp per query, 32 consecutive queries per CTA):
@@ -25,57 +24,19 @@
 
 namespace cl3d {
 
-// PseudoGrid influence of kernel point kp on relative position dp (:385-403), mask applied by caller
-__device__ __forceinline__ float pg_influence(float dx, float dy, float dz, const float* kp, int influence,
-                                              float inv_extent) {
-  if (influence == 1) return 1.f;  // 'constant'
-  const float ex = dx - kp[0], ey = dy - kp[1], ez = dz - kp[2];
-  const float sq = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez));
-  // clamp(1 - sqrt(sq)/extent, min=0) :397 ; torch's CUDA `tensor / python_scalar` multiplies by the fp32 reciprocal
-  const float h = 1.f - __fmul_rn(sqrtf(sq), inv_extent);
-  return h > 0.f ? h : 0.f;
-}
-
-// PseudoGrid staging with compaction: a slot whose influences are all zero (the neighbour is farther than
-// `extent` from every kernel point -- about 40 % of the slots of BASELINE c3, 2 of 15 influences non-zero on
-// average) contributes exact zeros to every sum, so it is not staged at all: no row gather, no FMAs.  The
-// surviving slots keep their order, so the result is bit-identical to the dense evaluation.
-// All 32 lanes call this; returns the number of staged slots.
-__device__ __forceinline__ int pg_stage_slots(float4* __restrict__ s_dp, float* __restrict__ s_h, int* __restrict__ s_m,
-                                              bool valid, float dx, float dy, float dz, unsigned row_off,
-                                              const float* __restrict__ kpts, int nkp, int influence, float inv_extent) {
-  float h[kMaxKP];
-  unsigned nz = 0;  // bit kp set <=> influence of kernel point kp is non-zero
-#pragma unroll
-  for (int kp = 0; kp < kMaxKP; ++kp) {
-    h[kp] = (valid && kp < nkp) ? pg_influence(dx, dy, dz, kpts + kp * 3, influence, inv_extent) : 0.f;
-    nz |= h[kp] > 0.f ? (1u << kp) : 0u;
-  }
-  const bool any = nz != 0;
-  const unsigned m = __ballot_sync(0xffffffffu, any);
-  if (any) {
-    const int pos = __popc(m & ((1u << lane_id()) - 1u));
-    s_dp[pos] = make_float4(dx, dy, dz, __uint_as_float(row_off));
-    s_m[pos] = (int)nz;
-    float4* h4 = reinterpret_cast<float4*>(s_h + (size_t)pos * kMaxKP);
-#pragma unroll
-    for (int k4 = 0; k4 < kMaxKP / 4; ++k4) h4[k4] = make_float4(h[4 * k4], h[4 * k4 + 1], h[4 * k4 + 2], h[4 * k4 + 3]);
-  }
-  return __popc(m);
-}
-
-template <int FAM>
-constexpr int rows_in_flight() {  // independent row loads per lane before they are consumed
-  return FAM == CL3D_FAM_PSEUDOGRID ? 2 : 4;
-}
 template <int FAM, bool BWD>
 constexpr int num_acc() {
-  return (FAM == CL3D_FAM_PSEUDOGRID && BWD) ? kMaxKP : ((BWD && FAM == CL3D_FAM_ADAPTIVE_DP) ? 4 : 1);
+  return (BWD && FAM == CL3D_FAM_ADAPTIVE_DP) ? 4 : 1;
 }
 
-// shared-memory carve-up (per CTA): per-warp slot arrays (dp + row index, influences / scales) + output tile
+// floats of s_h per slot.  Only the first is used (the backward's scale), but at a stride of 1 or 2 the compiler
+// schedules several backward kernels differently (agg_bwd_kernel<0, 4, *> grows from 648 to 768 instructions at 1);
+// at 4 their code differs from a wider stride only in shared-memory offsets.
+constexpr int kSlotH = 4;
+
+// shared-memory carve-up (per CTA): per-warp slot arrays (dp + row index, backward scale) + output tile
 struct SmemLayout {
-  size_t dp_off, h_off, m_off, out_off, red_off, total;
+  size_t dp_off, h_off, out_off, red_off, total;
 };
 __host__ __device__ inline SmemLayout smem_layout(int chunkC, int red_floats) {
   SmemLayout L;
@@ -83,9 +44,7 @@ __host__ __device__ inline SmemLayout smem_layout(int chunkC, int red_floats) {
   L.dp_off = o;
   o += (size_t)kAggWarps * kSlots * sizeof(float4);
   L.h_off = o;
-  o += (size_t)kAggWarps * kSlots * kMaxKP * sizeof(float);
-  L.m_off = o;
-  o += (size_t)kAggWarps * kSlots * sizeof(int);  // PseudoGrid: non-zero-influence bit mask per slot
+  o += (size_t)kAggWarps * kSlots * kSlotH * sizeof(float);
   L.out_off = o;
   o += (size_t)chunkC * (kTile + 1) * sizeof(float);
   o = align_up(o, 16);
@@ -95,45 +54,11 @@ __host__ __device__ inline SmemLayout smem_layout(int chunkC, int red_floats) {
   return L;
 }
 
-// one staged slot: applies the family to the row values v[CI] of that slot.
-// PseudoGrid forward uses  out[c] += f[c] * (sum_k' Wk[k',c] h[k'])  (one accumulator per channel, Wk in
-// registers); PseudoGrid backward accumulates T[k'][c] = sum_e g[c] h[k',e] (needed for d/dWk anyway).
-template <int FAM, int CI, bool BWD, int NACC, int NWK>
+// one staged slot: applies the family to the row values v[CI] of that slot; hk[0] is the backward's scale
+template <int FAM, int CI, bool BWD, int NACC>
 __device__ __forceinline__ void apply_slot(const float (&v)[CI], const float4& dp, const float* __restrict__ hk,
-                                           unsigned hmask, const float* __restrict__ s_wk_lane,
-                                           const LaneParams<FAM, CI>& lp, const float (&wk)[NWK][CI],
-                                           float (&acc)[NACC][CI]) {
-  if constexpr (FAM == CL3D_FAM_PSEUDOGRID && !BWD) {
-    // w[c] = sum over the NON-ZERO influences only (about 3 of 15, warp-uniform bit mask), ascending k' -- the
-    // skipped terms are exact zeros; kernel weights come from shared memory (dynamic k').
-    float w[CI];
-#pragma unroll
-    for (int i = 0; i < CI; ++i) w[i] = 0.f;
-    unsigned mm = hmask;
-    while (mm) {
-      const int kp = __ffs(mm) - 1;
-      mm &= mm - 1;
-      const float h = hk[kp];
-      const float* wrow = s_wk_lane + kp * (32 * CI);
-#pragma unroll
-      for (int i = 0; i < CI; ++i) w[i] = fmaf(h, wrow[32 * i], w[i]);
-    }
-#pragma unroll
-    for (int i = 0; i < CI; ++i) acc[0][i] = fmaf(v[i], w[i], acc[0][i]);
-  } else if constexpr (FAM == CL3D_FAM_PSEUDOGRID) {
-    const float4* h4 = reinterpret_cast<const float4*>(hk);
-#pragma unroll
-    for (int k4 = 0; k4 < kMaxKP / 4; ++k4) {
-      const float4 h = h4[k4];
-#pragma unroll
-      for (int i = 0; i < CI; ++i) {
-        acc[k4 * 4 + 0][i] = fmaf(h.x, v[i], acc[k4 * 4 + 0][i]);
-        acc[k4 * 4 + 1][i] = fmaf(h.y, v[i], acc[k4 * 4 + 1][i]);
-        acc[k4 * 4 + 2][i] = fmaf(h.z, v[i], acc[k4 * 4 + 2][i]);
-        acc[k4 * 4 + 3][i] = fmaf(h.w, v[i], acc[k4 * 4 + 3][i]);
-      }
-    }
-  } else if constexpr (BWD && FAM == CL3D_FAM_ADAPTIVE_DP) {
+                                           const LaneParams<FAM, CI>& lp, float (&acc)[NACC][CI]) {
+  if constexpr (BWD && FAM == CL3D_FAM_ADAPTIVE_DP) {
     const float sc = hk[0];  // 1/ncount (avg) or 1
 #pragma unroll
     for (int i = 0; i < CI; ++i) {
@@ -157,54 +82,26 @@ __device__ __forceinline__ void apply_slot(const float (&v)[CI], const float4& d
 // is the per-lane base pointer (matrix + chunk offset + lane): one IMAD.WIDE per row, then the CI loads use
 // immediate offsets (+32 floats each).  Lanes past the chunk read whatever follows (the next row, or the
 // CL3D_PM_SLACK floats every point-major buffer carries after its last row); their results are never stored.
-// Rows are loaded U at a time straight into registers (U*CI independent loads in flight per lane).
-template <int FAM, int CI, bool BWD, int NACC, int NWK>
-__device__ __forceinline__ void consume_slots(const float* __restrict__ lbase,
-                                              const float4* __restrict__ s_dp, const float* __restrict__ s_h,
-                                              const int* __restrict__ s_m, const float* __restrict__ s_wk_lane, int n,
-                                              const LaneParams<FAM, CI>& lp, const float (&wk)[NWK][CI],
+// Rows are loaded U = 4 at a time straight into registers (U*CI independent loads in flight per lane); these
+// kernels need few registers, so many resident warps hide the latency.
+template <int FAM, int CI, bool BWD, int NACC>
+__device__ __forceinline__ void consume_slots(const float* __restrict__ lbase, const float4* __restrict__ s_dp,
+                                              const float* __restrict__ s_h, int n, const LaneParams<FAM, CI>& lp,
                                               float (&acc)[NACC][CI]) {
-  constexpr bool MASKED = FAM == CL3D_FAM_PSEUDOGRID && !BWD;
-  constexpr int U = rows_in_flight<FAM>();
-  constexpr int HS = FAM == CL3D_FAM_PSEUDOGRID ? kMaxKP : 1;  // floats of s_h per slot
-  // software pipeline: group g+1 is loaded into the other register set while group g is consumed
-  auto load_group = [&](int s0, float4 (&dp)[U], float (&v)[U][CI]) {
+  constexpr int U = 4;
+  const int ng = n / U;
+  for (int g = 0; g < ng; ++g) {
+    float4 dp[U];
+    float v[U][CI];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      dp[u] = s_dp[s0 + u];
+      dp[u] = s_dp[g * U + u];
       const float* row = lbase + __float_as_uint(dp[u].w);
 #pragma unroll
       for (int i = 0; i < CI; ++i) v[u][i] = __ldg(row + 32 * i);  // lanes past the chunk read slack (unused)
     }
-  };
-  auto apply_group = [&](int s0, const float4 (&dp)[U], const float (&v)[U][CI]) {
 #pragma unroll
-    for (int u = 0; u < U; ++u)
-      apply_slot<FAM, CI, BWD, NACC, NWK>(v[u], dp[u], s_h + (size_t)(s0 + u) * HS, MASKED ? (unsigned)s_m[s0 + u] : 0u,
-                                          s_wk_lane, lp, wk, acc);
-  };
-  const int ng = n / U;
-  if constexpr (FAM == CL3D_FAM_PSEUDOGRID && BWD) {
-    // accumulator-heavy kernel (few resident warps): hide the row latency inside the warp
-    float4 dpA[U], dpB[U];
-    float vA[U][CI], vB[U][CI];
-    if (ng > 0) load_group(0, dpA, vA);
-    int g = 0;
-    for (; g + 2 <= ng; g += 2) {
-      load_group((g + 1) * U, dpB, vB);
-      apply_group(g * U, dpA, vA);
-      if (g + 2 < ng) load_group((g + 2) * U, dpA, vA);
-      apply_group((g + 1) * U, dpB, vB);
-    }
-    if (g < ng) apply_group(g * U, dpA, vA);
-  } else {
-    // light families: few registers, many resident warps hide the latency
-    for (int g = 0; g < ng; ++g) {
-      float4 dp[U];
-      float v[U][CI];
-      load_group(g * U, dp, v);
-      apply_group(g * U, dp, v);
-    }
+    for (int u = 0; u < U; ++u) apply_slot<FAM, CI, BWD, NACC>(v[u], dp[u], s_h + (size_t)(g * U + u), lp, acc);
   }
   for (int s = ng * U; s < n; ++s) {
     const float4 dp = s_dp[s];
@@ -212,7 +109,7 @@ __device__ __forceinline__ void consume_slots(const float* __restrict__ lbase,
     float v[CI];
 #pragma unroll
     for (int i = 0; i < CI; ++i) v[i] = __ldg(row + 32 * i);
-    apply_slot<FAM, CI, BWD, NACC, NWK>(v, dp, s_h + (size_t)s * HS, MASKED ? (unsigned)s_m[s] : 0u, s_wk_lane, lp, wk, acc);
+    apply_slot<FAM, CI, BWD, NACC>(v, dp, s_h + (size_t)s, lp, acc);
   }
 }
 
@@ -220,17 +117,15 @@ __device__ __forceinline__ void consume_slots(const float* __restrict__ lbase,
 // forward
 // =================================================================================================
 template <int FAM, int CI>
-__global__ void __launch_bounds__(kAggWarps * 32, FAM == CL3D_FAM_PSEUDOGRID ? 2 : 1) agg_fwd_kernel(const AggArgs a) {
+__global__ void __launch_bounds__(kAggWarps * 32, 1) agg_fwd_kernel(const AggArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c0 = blockIdx.y * 32 * CI;
   const int chunkC = min(32 * CI, a.Cp - c0);  // multiple of 8
   const SmemLayout L = smem_layout(32 * CI, 0);
   float4* s_dp = reinterpret_cast<float4*>(smem + L.dp_off) + (size_t)warp * kSlots;
-  float* s_h = reinterpret_cast<float*>(smem + L.h_off) + (size_t)warp * kSlots * kMaxKP;
-  int* s_m = reinterpret_cast<int*>(smem + L.m_off) + (size_t)warp * kSlots;
+  float* s_h = reinterpret_cast<float*>(smem + L.h_off) + (size_t)warp * kSlots * kSlotH;
   float* s_out = reinterpret_cast<float*>(smem + L.out_off);
-  float* s_wk = reinterpret_cast<float*>(smem + L.total);  // PseudoGrid: kernel weights [kMaxKP][32*CI]
 
   const int tiles_per_cloud = (a.M + kTile - 1) / kTile;
   const int b = blockIdx.x / tiles_per_cloud;
@@ -239,15 +134,6 @@ __global__ void __launch_bounds__(kAggWarps * 32, FAM == CL3D_FAM_PSEUDOGRID ? 2
   LaneParams<FAM, CI> lp;
   load_lane_params<FAM, CI>(lp, a, c0, lane);
   constexpr int NACC = num_acc<FAM, false>();
-  constexpr int NWK = 1;
-  const float wk[NWK][CI] = {};
-  if constexpr (FAM == CL3D_FAM_PSEUDOGRID) {
-    for (int e = threadIdx.x; e < kMaxKP * 32 * CI; e += blockDim.x) {
-      const int kp = e / (32 * CI), c = c0 + e % (32 * CI);
-      s_wk[e] = (kp < a.nkp && c < a.C) ? a.p1[(size_t)kp * a.C + c] : 0.f;
-    }
-    __syncthreads();
-  }
   const float* feat = a.feat_pm + (size_t)b * a.N * a.Cp + c0 + lane;  // per-lane base pointer
   const float* sxyz = a.support_xyz + (size_t)b * a.N * 3;
 
@@ -266,36 +152,20 @@ __global__ void __launch_bounds__(kAggWarps * 32, FAM == CL3D_FAM_PSEUDOGRID ? 2
 #pragma unroll
         for (int i = 0; i < CI; ++i) acc[s][i] = 0.f;
       for (int k0 = 0; k0 < nrows; k0 += kSlots) {
-        int rows = min(kSlots, nrows - k0);
-        // ---- stage: indices, relative positions (pt_utils.py:127-129), PseudoGrid influences
-        {
-          const bool valid = lane < rows;
-          float dx = 0.f, dy = 0.f, dz = 0.f;
-          unsigned roff = 0;
-          if (valid) {
-            const int j = a.idx[gq * a.K + k0 + lane];
-            const float3 d = rel_pos(a, sxyz[j * 3 + 0], sxyz[j * 3 + 1], sxyz[j * 3 + 2], qx, qy, qz);
-            dx = d.x, dy = d.y, dz = d.z;
-            roff = (unsigned)j * (unsigned)a.Cp;
-          }
-          if constexpr (FAM == CL3D_FAM_PSEUDOGRID) {
-            rows = pg_stage_slots(s_dp, s_h, s_m, valid, dx, dy, dz, roff, a.p0, a.nkp, a.influence, a.inv_extent);
-          } else {
-            if (valid) s_dp[lane] = make_float4(dx, dy, dz, __uint_as_float(roff));
-          }
+        const int rows = min(kSlots, nrows - k0);
+        // ---- stage: indices, relative positions (pt_utils.py:127-129)
+        if (lane < rows) {
+          const int j = a.idx[gq * a.K + k0 + lane];
+          const float3 d = rel_pos(a, sxyz[j * 3 + 0], sxyz[j * 3 + 1], sxyz[j * 3 + 2], qx, qy, qz);
+          s_dp[lane] = make_float4(d.x, d.y, d.z, __uint_as_float((unsigned)j * (unsigned)a.Cp));
         }
         __syncwarp();
-        consume_slots<FAM, CI, false, NACC, NWK>(feat, s_dp, s_h, s_m, s_wk + lane, rows, lp, wk, acc);
+        consume_slots<FAM, CI, false, NACC>(feat, s_dp, s_h, rows, lp, acc);
         __syncwarp();  // slots are rewritten by the next round / query
       }
-      if constexpr (FAM == CL3D_FAM_PSEUDOGRID) {
 #pragma unroll
-        for (int i = 0; i < CI; ++i) res[i] = acc[0][i];  // sum_m f[c,m] * sum_k' Wk[k',c] h[k',m]   (:415-419)
-      } else {
-#pragma unroll
-        for (int i = 0; i < CI; ++i)
-          res[i] = a.reduction == CL3D_REDUCE_AVG ? __fdiv_rn(acc[0][i], (float)nrows) : acc[0][i];  // :96-98
-      }
+      for (int i = 0; i < CI; ++i)
+        res[i] = a.reduction == CL3D_REDUCE_AVG ? __fdiv_rn(acc[0][i], (float)nrows) : acc[0][i];  // :96-98
     }
 #pragma unroll
     for (int i = 0; i < CI; ++i) s_out[(size_t)(lane + 32 * i) * (kTile + 1) + ql] = res[i];
@@ -308,49 +178,29 @@ __global__ void __launch_bounds__(kAggWarps * 32, FAM == CL3D_FAM_PSEUDOGRID ? 2
 // backward (gather form over the CSR lists)
 // =================================================================================================
 template <int FAM>
-__host__ __device__ constexpr int params_per_channel(int nkp) {
-  return FAM == CL3D_FAM_ADAPTIVE_DP ? 4 : (FAM == CL3D_FAM_PSEUDOGRID ? nkp : 0);
-}
-
-// PseudoGrid backward keeps its kernel weights and parameter-gradient accumulators in shared memory (they are
-// touched once per support point, not per neighbour), which halves the register count (2 CTAs per SM).
-__host__ __device__ inline size_t pg_bwd_extra_floats(int CI) {
-  return (size_t)kMaxKP * 32 * CI /*wk*/ + (size_t)kAggWarps * kMaxKP * 32 * CI /*per-warp pacc*/;
+__host__ __device__ constexpr int params_per_channel() {
+  return FAM == CL3D_FAM_ADAPTIVE_DP ? 4 : 0;
 }
 
 template <int FAM, int CI, typename TO>
-__global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID || CI > 3) ? 2 : 3) agg_bwd_kernel(const AggArgs a) {
+__global__ void __launch_bounds__(kAggWarps * 32, CI > 3 ? 2 : 3) agg_bwd_kernel(const AggArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c0 = blockIdx.y * 32 * CI;
   const int chunkC = min(32 * CI, a.Cp - c0);
   constexpr int NACC = num_acc<FAM, true>();
-  constexpr bool PG = FAM == CL3D_FAM_PSEUDOGRID;
   constexpr bool AW = FAM == CL3D_FAM_ADAPTIVE_DP;
-  const int ppc = params_per_channel<FAM>(a.nkp);
-  const SmemLayout L = smem_layout(32 * CI, ppc * 32 * CI);
+  const SmemLayout L = smem_layout(32 * CI, params_per_channel<FAM>() * 32 * CI);
   float4* s_dp = reinterpret_cast<float4*>(smem + L.dp_off) + (size_t)warp * kSlots;
-  float* s_h = reinterpret_cast<float*>(smem + L.h_off) + (size_t)warp * kSlots * kMaxKP;
-  int* s_m = reinterpret_cast<int*>(smem + L.m_off) + (size_t)warp * kSlots;
+  float* s_h = reinterpret_cast<float*>(smem + L.h_off) + (size_t)warp * kSlots * kSlotH;
   float* s_out = reinterpret_cast<float*>(smem + L.out_off);
   float* s_red = reinterpret_cast<float*>(smem + L.red_off);
-  float* s_wk = reinterpret_cast<float*>(smem + L.total);                 // [kMaxKP][32*CI]      (PG only)
-  float* s_pacc = s_wk + (size_t)kMaxKP * 32 * CI + (size_t)warp * kMaxKP * 32 * CI;  // per warp (PG only)
 
   LaneParams<FAM, CI> lp;
   load_lane_params<FAM, CI>(lp, a, c0, lane);
   bool ok[CI];
 #pragma unroll
   for (int i = 0; i < CI; ++i) ok[i] = lane + 32 * i < chunkC;
-  const float wk_dummy[1][CI] = {};
-  if constexpr (PG) {
-    for (int e = threadIdx.x; e < kMaxKP * 32 * CI; e += blockDim.x) {
-      const int kp = e / (32 * CI), c = c0 + e % (32 * CI);
-      s_wk[e] = (kp < a.nkp && c < a.C) ? a.p1[(size_t)kp * a.C + c] : 0.f;
-    }
-    for (int e = lane; e < kMaxKP * 32 * CI; e += 32) s_pacc[e] = 0.f;
-    __syncthreads();
-  }
   // AdaptiveWeight: per-lane parameter-gradient accumulators (x,y,z,bias) over all points this warp handles
   float pacc[AW ? 4 : 1][CI];
 #pragma unroll
@@ -384,43 +234,25 @@ __global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID ||
           for (int i = 0; i < CI; ++i) acc[s][i] = 0.f;
 
         for (int eb = e0; eb < e1; eb += kSlots) {
-          int rows = min(kSlots, e1 - eb);
-          {
-            const bool valid = lane < rows;
-            BwdEntry e = {0, make_float3(0.f, 0.f, 0.f), 0u};
-            if (valid) e = bwd_entry(a, qxyz, ent[eb + lane], px, py, pz);
-            if constexpr (PG) {
-              rows = pg_stage_slots(s_dp, s_h, s_m, valid, e.dp.x, e.dp.y, e.dp.z, e.roff, a.p0, a.nkp, a.influence,
-                                    a.inv_extent);
-            } else if (valid) {
-              s_dp[lane] = make_float4(e.dp.x, e.dp.y, e.dp.z, __uint_as_float(e.roff));
-              s_h[lane] = a.reduction == CL3D_REDUCE_AVG ? __fdiv_rn(1.f, (float)ncnt[e.q]) : 1.f;
-            }
+          const int rows = min(kSlots, e1 - eb);
+          if (lane < rows) {
+            const BwdEntry e = bwd_entry(a, qxyz, ent[eb + lane], px, py, pz);
+            s_dp[lane] = make_float4(e.dp.x, e.dp.y, e.dp.z, __uint_as_float(e.roff));
+            s_h[lane] = a.reduction == CL3D_REDUCE_AVG ? __fdiv_rn(1.f, (float)ncnt[e.q]) : 1.f;
           }
           __syncwarp();
-          consume_slots<FAM, CI, true, NACC, 1>(gpm, s_dp, s_h, s_m, nullptr, rows, lp, wk_dummy, acc);
+          consume_slots<FAM, CI, true, NACC>(gpm, s_dp, s_h, rows, lp, acc);
           __syncwarp();
         }
         // ---- epilogue: gradient w.r.t. this support point's features, parameter gradients
-        if constexpr (AW || PG) {
+        if constexpr (AW) {
           const float* frow = a.feat_pm + ((size_t)b * a.N + j) * a.Cp + c0 + lane;
 #pragma unroll
           for (int i = 0; i < CI; ++i) {
             const float f = ok[i] ? __ldg(frow + 32 * i) : 0.f;
-            if constexpr (AW) {
-              res[i] = fmaf(lp.c[i], acc[2][i], fmaf(lp.b[i], acc[1][i], fmaf(lp.a[i], acc[0][i], lp.d[i] * acc[3][i])));
+            res[i] = fmaf(lp.c[i], acc[2][i], fmaf(lp.b[i], acc[1][i], fmaf(lp.a[i], acc[0][i], lp.d[i] * acc[3][i])));
 #pragma unroll
-              for (int s = 0; s < 4; ++s) pacc[s][i] = fmaf(f, acc[s][i], pacc[s][i]);
-            } else {
-              float r = 0.f;
-#pragma unroll
-              for (int kp = 0; kp < kMaxKP; ++kp) {
-                const int o = kp * 32 * CI + lane + 32 * i;
-                r = fmaf(s_wk[o], acc[kp][i], r);
-                s_pacc[o] = fmaf(f, acc[kp][i], s_pacc[o]);  // this warp's private accumulator row
-              }
-              res[i] = r;
-            }
+            for (int s = 0; s < 4; ++s) pacc[s][i] = fmaf(f, acc[s][i], pacc[s][i]);
           }
         } else {
 #pragma unroll
@@ -436,18 +268,6 @@ __global__ void __launch_bounds__(kAggWarps * 32, (FAM == CL3D_FAM_PSEUDOGRID ||
   }
   // ---- CTA-level reduction of the parameter-gradient accumulators, fixed order over the warps
   if constexpr (AW) aw_bwd_params<CI>(a, pacc, s_red, c0);
-  if constexpr (PG) {
-    __syncthreads();
-    const float* all = s_wk + (size_t)kMaxKP * 32 * CI;  // [warps][kMaxKP][32*CI]
-    for (int e = threadIdx.x; e < ppc * 32 * CI; e += blockDim.x) {
-      float t = 0.f;
-#pragma unroll
-      for (int w = 0; w < kAggWarps; ++w) t += all[(size_t)w * kMaxKP * 32 * CI + e];
-      s_red[e] = t;
-    }
-    __syncthreads();
-    store_param_partial<CI>(a, s_red, ppc, c0);
-  }
 }
 
 // =================================================================================================
@@ -680,7 +500,7 @@ __global__ void __launch_bounds__(kAggWarps * 32, 3) sincos_bwd_kernel(const Agg
   const int F = a.C / 6;
   const SmemLayout L = smem_layout(2 * 32 * PI, 0);
   float4* s_dp = reinterpret_cast<float4*>(smem + L.dp_off) + (size_t)warp * kSlots;
-  float* s_h = reinterpret_cast<float*>(smem + L.h_off) + (size_t)warp * kSlots * kMaxKP;
+  float* s_h = reinterpret_cast<float*>(smem + L.h_off) + (size_t)warp * kSlots * kSlotH;
   float* s_out = reinterpret_cast<float*>(smem + L.out_off);
   PairLane<PI> pl;
   load_pair_lane<PI>(pl, a, p0, lane);
@@ -733,11 +553,10 @@ template <int FAM, int CI>
 static int launch_fwd(const AggArgs& a, cudaStream_t stream) {
   const int nchunks = ceil_div(a.Cp, 32 * CI);
   const SmemLayout L = smem_layout(32 * CI, 0);
-  const size_t smem = L.total + (FAM == CL3D_FAM_PSEUDOGRID ? (size_t)kMaxKP * 32 * CI * sizeof(float) : 0);
   static std::atomic<unsigned long long> seen{0};
   allow_big_smem(agg_fwd_kernel<FAM, CI>, seen);
   dim3 grid(a.ntiles, nchunks);
-  agg_fwd_kernel<FAM, CI><<<grid, kAggWarps * 32, smem, stream>>>(a);
+  agg_fwd_kernel<FAM, CI><<<grid, kAggWarps * 32, L.total, stream>>>(a);
   CL3D_LAUNCHED(1);
   return check_launch("agg_fwd_kernel");
 }
@@ -745,24 +564,21 @@ static int launch_fwd(const AggArgs& a, cudaStream_t stream) {
 template <int FAM, int CI>
 static int launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
   const int nchunks = ceil_div(a.Cp, 32 * CI);
-  const int ppc = params_per_channel<FAM>(a.nkp);
-  const SmemLayout L = smem_layout(32 * CI, ppc * 32 * CI);
-  const size_t smem = L.total + (FAM == CL3D_FAM_PSEUDOGRID ? pg_bwd_extra_floats(CI) * sizeof(float) : 0);
+  const SmemLayout L = smem_layout(32 * CI, params_per_channel<FAM>() * 32 * CI);
   dim3 grid(grid_x, nchunks);
   return with_dtype(a.out_dtype, [&](auto t) {
     using TO = typename decltype(t)::type;
     static std::atomic<unsigned long long> seen{0};
     allow_big_smem(agg_bwd_kernel<FAM, CI, TO>, seen);
-    agg_bwd_kernel<FAM, CI, TO><<<grid, kAggWarps * 32, smem, stream>>>(a);
+    agg_bwd_kernel<FAM, CI, TO><<<grid, kAggWarps * 32, L.total, stream>>>(a);
     CL3D_LAUNCHED(1);
     return check_launch("agg_bwd_kernel");
   });
 }
 
-static int pick_ci(int family, int Cp) {
-  int ci = ceil_div(Cp, 32);
-  const int cap = family == CL3D_FAM_PSEUDOGRID ? 3 : kMaxCI;  // PseudoGrid keeps nkp accumulators per channel
-  return ci > cap ? cap : ci;
+static int pick_ci(int Cp) {
+  const int ci = ceil_div(Cp, 32);
+  return ci > kMaxCI ? kMaxCI : ci;
 }
 
 #define DISPATCH_CI(FN, FAM, ...)                          \
@@ -773,12 +589,6 @@ static int pick_ci(int family, int Cp) {
     case 4: return FN<FAM, 4>(__VA_ARGS__);                \
     case 5: return FN<FAM, 5>(__VA_ARGS__);                \
     default: return FN<FAM, 6>(__VA_ARGS__);               \
-  }
-#define DISPATCH_CI3(FN, FAM, ...)                         \
-  switch (ci) {                                            \
-    case 1: return FN<FAM, 1>(__VA_ARGS__);                \
-    case 2: return FN<FAM, 2>(__VA_ARGS__);                \
-    default: return FN<FAM, 3>(__VA_ARGS__);               \
   }
 
 template <int PI>
@@ -817,7 +627,6 @@ static int dispatch_fwd(int family, int ci, const AggArgs& a, cudaStream_t s) {
     case CL3D_FAM_POSPOOL_XYZ: DISPATCH_CI(launch_fwd, CL3D_FAM_POSPOOL_XYZ, a, s)
     case CL3D_FAM_POSPOOL_SINCOS: return dispatch_sincos(a, false, a.ntiles, s);
     case CL3D_FAM_ADAPTIVE_DP: DISPATCH_CI(launch_fwd, CL3D_FAM_ADAPTIVE_DP, a, s)
-    case CL3D_FAM_PSEUDOGRID: DISPATCH_CI3(launch_fwd, CL3D_FAM_PSEUDOGRID, a, s)
   }
   return CL3D_ERR_UNSUPPORTED;
 }
@@ -826,7 +635,6 @@ static int dispatch_bwd(int family, int ci, const AggArgs& a, int gx, cudaStream
     case CL3D_FAM_POSPOOL_XYZ: DISPATCH_CI(launch_bwd, CL3D_FAM_POSPOOL_XYZ, a, gx, s)
     case CL3D_FAM_POSPOOL_SINCOS: return dispatch_sincos(a, true, gx, s);
     case CL3D_FAM_ADAPTIVE_DP: DISPATCH_CI(launch_bwd, CL3D_FAM_ADAPTIVE_DP, a, gx, s)
-    case CL3D_FAM_PSEUDOGRID: DISPATCH_CI3(launch_bwd, CL3D_FAM_PSEUDOGRID, a, gx, s)
   }
   return CL3D_ERR_UNSUPPORTED;
 }
@@ -905,9 +713,8 @@ extern "C" int cl3d_agg_fwd(int family, int reduction, const float* feat_pm, con
   a.ntiles = B * ceil_div(M, kTile);
   a.arg_pm = arg_pm;
   if (reduction == CL3D_REDUCE_MAX) return aggmax_launch(family, a, false, a.ntiles, (cudaStream_t)stream_);
-  if (family == CL3D_FAM_PSEUDOGRID && pg3_fwd_supported(a)) return pg3_launch_fwd(a, (cudaStream_t)stream_);
-  if (family == CL3D_FAM_PSEUDOGRID && pg2_supported(a)) return pg2_launch_fwd(a, (cudaStream_t)stream_);
-  return dispatch_fwd(family, pick_ci(family, a.Cp), a, (cudaStream_t)stream_);
+  if (family == CL3D_FAM_PSEUDOGRID) return pg_launch(a, false, a.ntiles, (cudaStream_t)stream_);
+  return dispatch_fwd(family, pick_ci(a.Cp), a, (cudaStream_t)stream_);
 }
 
 extern "C" int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const float* feat_pm,
@@ -942,9 +749,6 @@ extern "C" int cl3d_agg_bwd(int family, int reduction, const float* g_pm, const 
   a.ntiles = B * ceil_div(N, kTile);
   a.arg_pm = const_cast<unsigned char*>(arg_pm);
   if (reduction == CL3D_REDUCE_MAX) return aggmax_launch(family, a, true, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
-  if (family == CL3D_FAM_PSEUDOGRID && pg3_supported(a))
-    return pg3_launch_bwd(a, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
-  if (family == CL3D_FAM_PSEUDOGRID && pg2_supported(a))
-    return pg2_launch_bwd(a, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
-  return dispatch_bwd(family, pick_ci(family, a.Cp), a, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
+  if (family == CL3D_FAM_PSEUDOGRID) return pg_launch(a, true, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
+  return dispatch_bwd(family, pick_ci(a.Cp), a, bwd_grid_x(a.ntiles), (cudaStream_t)stream_);
 }

@@ -117,7 +117,8 @@ __device__ __forceinline__ BwdEntry bwd_entry(const AggArgs& a, const float* qxy
   return e;
 }
 
-// this CTA's rows of the parameter-gradient partials (gridDim.x, ppc, C), from s_red[ppc][32*CI]
+// this CTA's rows of the parameter-gradient partials (gridDim.x, ppc, C), from s_red[ppc][32*CI]; aw_bwd_params
+// writes AdaptiveWeight's four rows per channel through it
 template <int CI>
 __device__ __forceinline__ void store_param_partial(const AggArgs& a, const float* s_red, int ppc, int c0) {
   for (int e = threadIdx.x; e < ppc * 32 * CI; e += blockDim.x) {
@@ -206,17 +207,9 @@ __device__ __forceinline__ void aw_bwd_params(const AggArgs& a, const float (&pa
 }
 
 
-// pg.cu: PseudoGrid forward / backward, float4 lanes + packed fp32 FMA + sparse kernel-point walk.
-// Return CL3D_ERR_UNSUPPORTED when the shape is outside their range (the caller then uses the generic kernels).
-int pg2_launch_fwd(const AggArgs& a, cudaStream_t stream);
-int pg2_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream);
-bool pg2_supported(const AggArgs& a);
-// third generation (tensor-core accumulation per kernel point): forward for the shapes pg3_fwd_supported accepts,
-// backward for those of pg3_supported; backward: grid_x = rows of a.partial the caller sums
-int pg3_launch_fwd(const AggArgs& a, cudaStream_t stream);
-int pg3_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream);
-bool pg3_supported(const AggArgs& a);
-bool pg3_fwd_supported(const AggArgs& a);
+// pg.cu: PseudoGrid forward / backward (sum reduction); picks the tensor-core kernel where it serves the shape, the
+// general one otherwise.  Forward: grid_x = a.ntiles; backward: grid_x = rows of a.partial the caller sums
+int pg_launch(const AggArgs& a, bool bwd, int grid_x, cudaStream_t stream);
 
 // agg_max.cu: max reduction for PosPool (xyz | sin_cos) and AdaptiveWeight
 int aggmax_launch(int family, const AggArgs& a, bool bwd, int grid_x, cudaStream_t stream);

@@ -10,20 +10,18 @@
 // ONE kernel template serves both directions: centre point p (query / support point), a list of neighbour rows
 // (features / upstream gradients).
 //
-// Why a second generation.  The first one (agg.cu) spends most of its forward instructions on influences (16 scalar
-// IEEE square roots per neighbour) and on walking the (neighbour, kernel point) pairs at 15 instructions per pair (bit
-// scan + two address computations + three 4-byte weight loads + three scalar FMAs), plus shuffle reductions of the
-// BatchNorm partials; its backward keeps 16 accumulators per channel (127 registers).  Here:
+// pg2_kernel.  Its instructions go to the influences (16 per neighbour) and to the walk over the (neighbour, kernel
+// point) pairs, so both are kept short, and one accumulator per channel keeps the registers down:
 //   * a lane owns 4 CONSECUTIVE channels: one 16-byte load per neighbour row / weight row, arithmetic in channel
 //     pairs (FMAs with a scalar-broadcast h operand);
 //   * staging compiles, per neighbour with any non-zero influence, a list of (h, weight-row byte offset) entries
 //     -- 40 % of the neighbours have none and are dropped, the others ~3 of 15 -- so the pair loop is
-//     {8-byte entry load, 16-byte weight load, 4 FFMA, branch}: 7 instructions instead of 15;
+//     {8-byte entry load, 16-byte weight load, 4 FFMA, branch}: 7 instructions per pair;
 //   * influences are evaluated straight-line and packed (two kernel points per instruction), the square root with
 //     the hardware approximation (2^-22 relative: h moves by < 3e-7, far inside the 1e-5 parity bar);
 //   * BatchNorm partial moments are taken once per tile from the output tile in shared memory;
 //   * the backward uses the same one-accumulator w-form for d/df and adds d/dWk into a per-warp shared-memory
-//     accumulator addressed by the entry's offset: ~64 registers instead of 127.
+//     accumulator addressed by the entry's offset (~64 registers; 16 register accumulators per channel took 127).
 // One warp per centre point, 32 centre points per CTA tile; the backward is a persistent tile loop.
 //
 // Not shipped: kernel weights and d/dWk accumulators resident in registers with dense kernel-point quads on the FMA
@@ -98,8 +96,8 @@ __device__ __forceinline__ void load_xyz(const float* __restrict__ xyz, int r, f
 }
 
 // The 16 influences of one neighbour at relative position (dx, dy, dz) (reference :385-398: sq = |dp - K|^2,
-// h = clamp(1 - sqrt(sq)/extent, 0); 'constant': 1), two kernel points per instruction.  Every generation of the
-// kernel takes its influences from here, so they agree bit for bit.
+// h = clamp(1 - sqrt(sq)/extent, 0); 'constant': 1), two kernel points per instruction.  pg2_kernel and pg3_body
+// both take their influences from here, so they agree bit for bit.
 __device__ __forceinline__ void pg_influences(float (&h)[kMaxKP], bool valid, float dx, float dy, float dz,
                                               const u64* __restrict__ s_kx, const u64* __restrict__ s_ky,
                                               const u64* __restrict__ s_kz, int nkp, int influence, float inv_extent) {
@@ -215,9 +213,8 @@ __device__ __forceinline__ void pg_consume(const float* __restrict__ rows, uint3
   }
 }
 
-// Layers wider than 128 channels run as gridDim.y channel chunks of equal width (a multiple of 4, <= 128): every
-// chunk stages the influences again -- as the first generation does per 96 channels -- but keeps this kernel's
-// cheaper pair loop.
+// Layers wider than 128 channels (32 lanes of 4 channels) run as gridDim.y channel chunks of equal width (a multiple
+// of 4, <= 128); every chunk stages the influences again.
 __host__ __device__ inline int pg_num_chunks(int Cp) { return (Cp + 127) / 128; }
 __host__ __device__ inline int pg_chunk_width(int Cp, int nchunks) { return ((Cp + nchunks - 1) / nchunks + 3) / 4 * 4; }
 
@@ -780,16 +777,15 @@ __global__ void __launch_bounds__(kPgWarps * 32, kPg3CtasPerSM) pg3_bwd_kernel(c
 // Third generation: up to 72 padded channels in one chunk, or two equal chunks up to 128.
 // CL3D_PG_V2 forces the second generation in both directions (A/B measurements, tests).
 static int pg3_num_chunks(int Cp) { return Cp <= 8 * kPg3MaxNT ? 1 : 2; }
-bool pg3_supported(const AggArgs& a) {
-  if (getenv("CL3D_PG_V1") || getenv("CL3D_PG_V2")) return false;
-  if (a.nkp < 1 || a.nkp > kMaxKP || a.Cp > 128) return false;
+static bool pg3_supported(const AggArgs& a) {
+  if (getenv("CL3D_PG_V2") || a.Cp > 128) return false;
   return a.Cp % (8 * pg3_num_chunks(a.Cp)) == 0;
 }
 // The forward takes the third generation only up to 40 padded channels: measured on H100 (DESIGN.md 7.1) it beats
 // pg2_kernel<false> at 36 channels but loses at 72 and 128, where its row staging at 2 CTAs per SM costs more than
-// pg2's weight-row loads at 4.
+// pg2's weight-row loads at 4.  That is one chunk, so the forward is instantiated for NT <= kPg3FwdMaxCp / 8 only.
 constexpr int kPg3FwdMaxCp = 40;
-bool pg3_fwd_supported(const AggArgs& a) { return a.Cp <= kPg3FwdMaxCp && pg3_supported(a); }
+static bool pg3_fwd_supported(const AggArgs& a) { return a.Cp <= kPg3FwdMaxCp && pg3_supported(a); }
 
 template <bool BWD, int NT>
 static void pg3_launch_nt(const AggArgs& a, dim3 grid, int partial_rows, cudaStream_t stream) {
@@ -808,65 +804,48 @@ static void pg3_launch_nt(const AggArgs& a, dim3 grid, int partial_rows, cudaStr
   }
 }
 
-template <bool BWD>
-static void pg3_launch(const AggArgs& a, dim3 grid, int partial_rows, cudaStream_t stream) {
-  switch (a.Cp / (8 * pg3_num_chunks(a.Cp))) {
-    case 1: pg3_launch_nt<BWD, 1>(a, grid, partial_rows, stream); break;
-    case 2: pg3_launch_nt<BWD, 2>(a, grid, partial_rows, stream); break;
-    case 3: pg3_launch_nt<BWD, 3>(a, grid, partial_rows, stream); break;
-    case 4: pg3_launch_nt<BWD, 4>(a, grid, partial_rows, stream); break;
-    case 5: pg3_launch_nt<BWD, 5>(a, grid, partial_rows, stream); break;
-    case 6: pg3_launch_nt<BWD, 6>(a, grid, partial_rows, stream); break;
-    case 7: pg3_launch_nt<BWD, 7>(a, grid, partial_rows, stream); break;
-    case 8: pg3_launch_nt<BWD, 8>(a, grid, partial_rows, stream); break;
-    default: pg3_launch_nt<BWD, 9>(a, grid, partial_rows, stream); break;
-  }
+// the instance for nt 8-channel tiles per chunk, NT_MAX for nt >= NT_MAX
+template <bool BWD, int NT_MAX>
+static void pg3_launch(int nt, const AggArgs& a, dim3 grid, int partial_rows, cudaStream_t stream) {
+  if constexpr (NT_MAX > 1)
+    if (nt < NT_MAX) return pg3_launch<BWD, NT_MAX - 1>(nt, a, grid, partial_rows, stream);
+  pg3_launch_nt<BWD, NT_MAX>(a, grid, partial_rows, stream);
 }
 
 // one wave of resident CTAs looping over the 32-query tiles (CL3D_TEST_MAX_GRID caps it)
-int pg3_launch_fwd(const AggArgs& a, cudaStream_t stream) {
-  if (!pg3_fwd_supported(a)) return CL3D_ERR_UNSUPPORTED;
+static int pg3_launch_fwd(const AggArgs& a, cudaStream_t stream) {
   const int gx = max(1, min(a.ntiles, min(kPg3CtasPerSM * sm_count(), persistent_grid_cap())));
-  pg3_launch<false>(a, dim3(gx, pg3_num_chunks(a.Cp)), 0, stream);
+  pg3_launch<false, kPg3FwdMaxCp / 8>(a.Cp / 8, a, dim3(gx, 1), 0, stream);
   CL3D_LAUNCHED(1);
   return check_launch("pg3_fwd_kernel");
 }
 
 // grid_x = rows of a.partial the caller sums; the kernel runs one wave of resident CTAs
-int pg3_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
-  if (!pg3_supported(a)) return CL3D_ERR_UNSUPPORTED;
-  const dim3 grid(min(grid_x, kPg3CtasPerSM * sm_count()), pg3_num_chunks(a.Cp));
-  pg3_launch<true>(a, grid, grid_x, stream);
+static int pg3_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
+  const int nchunks = pg3_num_chunks(a.Cp);
+  const dim3 grid(min(grid_x, kPg3CtasPerSM * sm_count()), nchunks);
+  pg3_launch<true, kPg3MaxNT>(a.Cp / (8 * nchunks), a, grid, grid_x, stream);
   CL3D_LAUNCHED(1);
   return check_launch("pg3_bwd_kernel");
 }
 
-bool pg2_supported(const AggArgs& a) {
-  if (getenv("CL3D_PG_V1")) return false;  // A/B switch: first-generation kernels (tests, profiling)
-  return a.nkp >= 1 && a.nkp <= kMaxKP;
-}
-
-int pg2_launch_fwd(const AggArgs& a, cudaStream_t stream) {
-  if (!pg2_supported(a)) return CL3D_ERR_UNSUPPORTED;
-
+static int pg2_launch_fwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
   const int nchunks = pg_num_chunks(a.Cp);
   const PgSmem L = pg_smem(pg_chunk_width(a.Cp, nchunks), false);
   static std::atomic<unsigned long long> seen{0};
   if (nchunks == 1) {
     allow_big_smem(pg2_kernel<false, false, float>, seen);
-    pg2_kernel<false, false, float><<<a.ntiles, kPgWarps * 32, L.total, stream>>>(a);
+    pg2_kernel<false, false, float><<<grid_x, kPgWarps * 32, L.total, stream>>>(a);
   } else {
     static std::atomic<unsigned long long> seen_c{0};
     allow_big_smem(pg2_kernel<false, true, float>, seen_c);
-    pg2_kernel<false, true, float><<<dim3(a.ntiles, nchunks), kPgWarps * 32, L.total, stream>>>(a);
+    pg2_kernel<false, true, float><<<dim3(grid_x, nchunks), kPgWarps * 32, L.total, stream>>>(a);
   }
   CL3D_LAUNCHED(1);
   return check_launch("pg2_kernel<fwd>");
 }
 
-int pg2_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
-  if (!pg2_supported(a)) return CL3D_ERR_UNSUPPORTED;
-
+static int pg2_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
   const int nchunks = pg_num_chunks(a.Cp);
   const PgSmem L = pg_smem(pg_chunk_width(a.Cp, nchunks), true);
   with_dtype(a.out_dtype, [&](auto t) {
@@ -884,6 +863,11 @@ int pg2_launch_bwd(const AggArgs& a, int grid_x, cudaStream_t stream) {
   });
   CL3D_LAUNCHED(1);
   return check_launch("pg2_kernel<bwd>");
+}
+
+int pg_launch(const AggArgs& a, bool bwd, int grid_x, cudaStream_t stream) {
+  if (bwd) return pg3_supported(a) ? pg3_launch_bwd(a, grid_x, stream) : pg2_launch_bwd(a, grid_x, stream);
+  return pg3_fwd_supported(a) ? pg3_launch_fwd(a, stream) : pg2_launch_fwd(a, grid_x, stream);
 }
 
 }  // namespace cl3d

@@ -41,21 +41,20 @@ SINCOS = lambda red: dict(pospool=dict(position_embedding="sin_cos", reduction=r
 AW = lambda red: dict(adaptive_weight=dict(weight_type="dp", num_mlps=1, shared_channels=1, reduction=red))  # noqa
 PW = dict(pointwisemlp=dict(feature_type="dp_fi_df", num_mlps=1, reduction="max"))
 
-# one case per producer of BatchNorm partials: id -> (la_type, config override, C, environment)
+# one case per producer of BatchNorm partials: id -> (la_type, config override, C)
 CASES = {
-    "agg-xyz-avg": ("pospool", XYZ("avg"), 24, {}),
-    "agg-xyz-sum": ("pospool", XYZ("sum"), 24, {}),
-    "agg-aw-avg": ("adaptive_weight", AW("avg"), 24, {}),
-    "agg-pg-v1": ("pseudo_grid", {}, 72, {"CL3D_PG_V1": "1"}),
-    "sincos-avg": ("pospool", SINCOS("avg"), 24, {}),
-    "aggmax-xyz": ("pospool", XYZ("max"), 24, {}),
-    "aggmax-sincos": ("pospool", SINCOS("max"), 24, {}),
-    "aggmax-aw": ("adaptive_weight", AW("max"), 24, {}),
-    "pg2-72": ("pseudo_grid", {}, 72, {}),
-    "pg2-144": ("pseudo_grid", {}, 144, {}),          # two channel chunks
-    "pg3-36": ("pseudo_grid", {}, 36, {}),
-    "pwmlp-72": ("pointwisemlp", PW, 72, {}),
-    "pwmlp-160": ("pointwisemlp", PW, 160, {}),       # two output chunks of the forward
+    "agg-xyz-avg": ("pospool", XYZ("avg"), 24),
+    "agg-xyz-sum": ("pospool", XYZ("sum"), 24),
+    "agg-aw-avg": ("adaptive_weight", AW("avg"), 24),
+    "sincos-avg": ("pospool", SINCOS("avg"), 24),
+    "aggmax-xyz": ("pospool", XYZ("max"), 24),
+    "aggmax-sincos": ("pospool", SINCOS("max"), 24),
+    "aggmax-aw": ("adaptive_weight", AW("max"), 24),
+    "pg2-72": ("pseudo_grid", {}, 72),
+    "pg2-144": ("pseudo_grid", {}, 144),          # two channel chunks
+    "pg3-36": ("pseudo_grid", {}, 36),
+    "pwmlp-72": ("pointwisemlp", PW, 72),
+    "pwmlp-160": ("pointwisemlp", PW, 160),       # two output chunks of the forward
 }
 RATIOS = [1e2, 1e3, 1e4]
 B, N, K = 2, 48, 16
@@ -152,14 +151,13 @@ def values64(call):
 
 
 def run_forward(cuda, case, M, target, seed, padded=False, const_channel=False, monkeypatch=None, lam=None):
-    la_type, over, C, envs = CASES[case]
+    la_type, over, C = CASES[case]
 
     def once(lam):
         r, q, s, qm, sm, feats = make_inputs(C, M, lam, seed, padded, const_channel)
         mod = make_module(la_type, over, C, r, seed, const_channel).to(cuda).train()
         cap = Capture(monkeypatch)
-        with env(**envs):
-            mod(q.to(cuda), s.to(cuda), qm.to(cuda), sm.to(cuda), feats.to(cuda))
+        mod(q.to(cuda), s.to(cuda), qm.to(cuda), sm.to(cuda), feats.to(cuda))
         torch.cuda.synchronize()
         monkeypatch.undo()
         assert len(cap.calls) == 1
@@ -251,10 +249,10 @@ def _rel(a, b):
 
 
 @pytest.mark.parametrize("target", RATIOS, ids=lambda t: f"ratio{t:.0e}")
-@pytest.mark.parametrize("case", [c for c in CASES if not CASES[c][3]])
+@pytest.mark.parametrize("case", list(CASES))
 def test_module_large_mean_matches_f64_like_fp32_reference(cuda, monkeypatch, case, target):
     from oracle import f64_ext, la_oracle
-    la_type, over, C, envs = CASES[case]
+    la_type, over, C = CASES[case]
     _, _, _, rho = run_forward(cuda, case, M_ODD, target, 31, monkeypatch=monkeypatch)
     r, q, s, qm, sm, feats = make_inputs(C, M_ODD, rho, 31)
     mod = make_module(la_type, over, C, r, 31)
@@ -329,7 +327,7 @@ def test_module_large_mean_matches_f64_like_fp32_reference(cuda, monkeypatch, ca
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("case", list(CASES))
 def test_bn_partials_repeat_and_graph_replay(cuda, monkeypatch, case):
-    la_type, over, C, envs = CASES[case]
+    la_type, over, C = CASES[case]
     call, x, ratio, rho = run_forward(cuda, case, M_ODD, 1e3, 41, monkeypatch=monkeypatch)
     call2, _, _, _ = run_forward(cuda, case, M_ODD, 1e3, 41, monkeypatch=monkeypatch, lam=rho)
     assert torch.equal(call["partial"], call2["partial"]), "two runs give different partials"
@@ -355,28 +353,26 @@ def test_bn_partials_repeat_and_graph_replay(cuda, monkeypatch, case):
 
     fwd = ops.agg_fwd
     monkeypatch.setattr(ops, "agg_fwd", rec)
-    with env(**envs):
-        mod(q.to(cuda), s.to(cuda), qm.to(cuda), sm.to(cuda), feats.to(cuda))
+    mod(q.to(cuda), s.to(cuda), qm.to(cuda), sm.to(cuda), feats.to(cuda))
     monkeypatch.undo()
     a, k = args[0]
-    with env(**envs):
-        eager_agg, eager_part = fwd(*a, **k)
-        eager = fin(eager_part, *st[2])
-        torch.cuda.synchronize()
-        rm, rv = torch.zeros(C, device=cuda), torch.ones(C, device=cuda)
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            fin(fwd(*a, **k)[1], rm.clone(), rv.clone())
-        torch.cuda.current_stream().wait_stream(side)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            g_agg, g_part = fwd(*a, **k)
-            g_stats = fin(g_part, rm, rv)
-        g_agg.zero_()
-        g_part.zero_()
-        g_stats.zero_()
-        graph.replay()
-        torch.cuda.synchronize()
+    eager_agg, eager_part = fwd(*a, **k)
+    eager = fin(eager_part, *st[2])
+    torch.cuda.synchronize()
+    rm, rv = torch.zeros(C, device=cuda), torch.ones(C, device=cuda)
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        fin(fwd(*a, **k)[1], rm.clone(), rv.clone())
+    torch.cuda.current_stream().wait_stream(side)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        g_agg, g_part = fwd(*a, **k)
+        g_stats = fin(g_part, rm, rv)
+    g_agg.zero_()
+    g_part.zero_()
+    g_stats.zero_()
+    graph.replay()
+    torch.cuda.synchronize()
     assert torch.equal(g_agg, eager_agg) and torch.equal(g_part, eager_part) and torch.equal(g_stats, eager)
     assert torch.equal(rm, st[2][0]) and torch.equal(rv, st[2][1])

@@ -89,10 +89,15 @@ def test_pg_v3_fwd_matches_v2_and_f64(cuda, B, N, K, C, nkp, influence, thin, ma
     def sums(m):   # (ntiles, 2, C): sum and sum of squares
         return torch.stack([m[:, 1], m[:, 2] + m[:, 1] ** 2 / m[:, 0]], 1)
 
-    ep = max(_err(sums(m3), sums(mref)), _err(m3[:, 2], _tile_moments(a3)[:, 2]))
-    print(f"float64 reference: agg v2 {e2:.2e} v3 {e3:.2e} | v3 BatchNorm partials {ep:.2e}")
+    assert torch.equal(m2[:, 0], mref[:, 0])
+    ep2 = max(_err(sums(m2), sums(mref)), _err(m2[:, 2], _tile_moments(a2)[:, 2]))
+    ep3 = max(_err(sums(m3), sums(mref)), _err(m3[:, 2], _tile_moments(a3)[:, 2]))
+    print(f"float64 reference: agg v2 {e2:.2e} v3 {e3:.2e} | BatchNorm partials v2 {ep2:.2e} v3 {ep3:.2e}")
+    assert e2 <= 5e-6, f"agg: v2 differs from float64 by {e2:.2e}"
+    assert e3 <= 5e-6, f"agg: default dispatch differs from float64 by {e3:.2e}"
     assert e3 <= max(3 * e2, 2e-6), f"v3 {e3:.2e} against v2 {e2:.2e}"
-    assert ep <= 1e-5
+    assert ep2 <= 1e-5, f"BatchNorm partials: v2 differ from float64 by {ep2:.2e}"
+    assert ep3 <= 1e-5, f"BatchNorm partials: default dispatch differs from float64 by {ep3:.2e}"
     # BatchNorm statistics from the partials, as cl3d_bn_finalize merges them
     s2, s3 = _stats(p2, C, B * N), _stats(p3, C, B * N)
     assert float((s3 - s2).abs().max()) <= 1e-5 * max(1.0, float(s2.abs().max()))

@@ -405,11 +405,10 @@ def _padded(C):
     return (C + 7) & ~7
 
 
-def agg_instance(C, pg=False):
-    """agg.cu:851-855 pick_ci (cap kMaxCI = 6, agg_common.cuh:10; PseudoGrid 3) and launch_fwd's chunk count
-    (agg.cu:826) -> (CI, chunks)"""
+def agg_instance(C):
+    """agg.cu pick_ci (cap kMaxCI = 6, agg_common.cuh) and launch_fwd's chunk count -> (CI, chunks)"""
     Cp = _padded(C)
-    ci = min(_cdiv(Cp, 32), 3 if pg else 6)
+    ci = min(_cdiv(Cp, 32), 6)
     return ci, _cdiv(Cp, 32 * ci)
 
 

@@ -9,8 +9,8 @@ from closerlook3d_b200.config import baseline_config
 MAP = [("gemm_tf32x3", "cl3d_sgemm_algo"), ("sgemm", "cl3d_sgemm_algo"), ("splitk_reduce", "cl3d_sgemm_algo"),
        ("ball_query", "cl3d_ball_query_csr"), ("grid_build_fused", "cl3d_ball_query_csr"), ("csr_", "cl3d_ball_query_csr"),
        ("pg2_kernel<(bool)0", "cl3d_agg_fwd"), ("pg2_kernel<(bool)1", "cl3d_agg_bwd"), ("pg2_kernel<0", "cl3d_agg_fwd"),
-       ("pg2_kernel<1", "cl3d_agg_bwd"), ("pg3_bwd_kernel", "cl3d_agg_bwd"), ("aggmax_fwd", "cl3d_agg_fwd"),
-       ("aggmax_bwd", "cl3d_agg_bwd"), ("nearest_query", "cl3d_nearest_query"),
+       ("pg2_kernel<1", "cl3d_agg_bwd"), ("pg3_bwd_kernel", "cl3d_agg_bwd"), ("pg3_fwd_kernel", "cl3d_agg_fwd"),
+       ("aggmax_fwd", "cl3d_agg_fwd"), ("aggmax_bwd", "cl3d_agg_bwd"), ("nearest_query", "cl3d_nearest_query"),
        ("pwmlp_fwd_kernel", "cl3d_pwmlp_fwd_stats"), ("pwmlp_out", "cl3d_pwmlp_fwd_out"), ("pwmlp_bwd", "cl3d_pwmlp_bwd"),
        ("agg_fwd", "cl3d_agg_fwd"), ("sincos_fwd", "cl3d_agg_fwd"), ("agg_bwd", "cl3d_agg_bwd"), ("sincos_bwd", "cl3d_agg_bwd"),
        ("bn_relu_fwd", "cl3d_bn_relu_fwd"), ("bn_relu_bwd", "cl3d_bn_relu_bwd"), ("bn_reduce2", "cl3d_bn_relu_bwd"),
