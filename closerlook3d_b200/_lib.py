@@ -56,7 +56,6 @@ SIGNATURES = {
     "cl3d_pwmlp_weight_grad": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
     "cl3d_to_point_major_aug": (_i, [_vp, _i, _vp, _i, _i, _i, _f, _vp, _vp]),
     "cl3d_pwmlp_fwd_stats": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "cl3d_pwmlp_fwd_out": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp]),
     "cl3d_pwmlp_bwd_scratch_floats": (_sz, [_i, _i, _i, _i, _i]),
     "cl3d_pwmlp_bwd": (_i, [_vp, _i] + [_vp] * 15 + [_i, _i, _i, _i, _i, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "cl3d_mhead_save_floats": (_sz, [_i, _i]),

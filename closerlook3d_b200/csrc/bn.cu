@@ -6,13 +6,12 @@
 // Batch statistics come from the per-tile moments the aggregation kernel already produced, so the
 // forward costs one read + one write of (B,C,M); the backward is two passes (statistics, apply) and writes
 // d(loss)/d(agg) directly in the point-major layout the gather-form aggregation backward consumes.
+// PointWiseMLP's output relu(BN2d(ysel)) is the same forward over its selected extremum ysel (B,Cout,M).
 #include <type_traits>
 
 #include "common.cuh"
 
 namespace cl3d {
-
-constexpr int kBnTile = 32;
 
 // one tile's moments (store_bn_moments) added to the sums of (x - shift) and (x - shift)^2: with g = centre - shift,
 //   sum (x - shift) = d + n g,   sum (x - shift)^2 = q + 2 g d + n g^2
@@ -96,7 +95,7 @@ __global__ void __launch_bounds__(256) bn_relu_fwd_kernel(const float* __restric
   const float* xr = x + (size_t)row * M;
   T* yr = y + (size_t)row * M;
   for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < M; i += gridDim.y * blockDim.x) {
-    const float v = __fmaf_rn(__fsub_rn(xr[i], mean), sc, sh);  // the backward recomputes exactly this
+    const float v = bn_preact(xr[i], mean, sc, sh);
     store_f32(yr + i, v > 0.f ? v : 0.f);
   }
 }
@@ -118,7 +117,7 @@ __device__ __forceinline__ void load4(const T* __restrict__ p, int q, int M, boo
   }
 }
 
-// pass 1: per tile and channel: sum(gy), sum(gy * xhat)
+// pass 1: per tile and channel: sum(gy * xhat), sum(gy) -- rows (dgamma, dbeta) for cl3d_reduce_partials
 template <typename T>
 __global__ void __launch_bounds__(256) bn_relu_bwd_stats_kernel(const T* __restrict__ grad_y,
                                                                 const float* __restrict__ x,
@@ -141,17 +140,15 @@ __global__ void __launch_bounds__(256) bn_relu_bwd_stats_kernel(const T* __restr
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
       if (q + t < M) {
-        const float xc = __fsub_rn(xv[t], mean);
-        const float yv = __fmaf_rn(xc, sc, sh);  // bit-identical to the forward's y
-        const float g = yv > 0.f ? gv[t] : 0.f;
+        const float g = bn_preact(xv[t], mean, sc, sh) > 0.f ? gv[t] : 0.f;
         gy += g;
-        gx = fmaf(g, xc * invstd, gx);
+        gx = fmaf(g, __fsub_rn(xv[t], mean) * invstd, gx);
       }
     }
     const float s1 = warp_sum(gy), s2 = warp_sum(gx);
     if (lane == 0) {
-      partial[((size_t)blockIdx.x * 2 + 0) * C + c] = s1;
-      partial[((size_t)blockIdx.x * 2 + 1) * C + c] = s2;
+      partial[((size_t)blockIdx.x * 2 + 0) * C + c] = s2;
+      partial[((size_t)blockIdx.x * 2 + 1) * C + c] = s1;
     }
   }
 }
@@ -188,10 +185,8 @@ __global__ void __launch_bounds__(256) bn_relu_bwd_apply_kernel(const T* __restr
         const float mg = training ? dgb[C + c] * inv_count : 0.f, mgx = training ? dgb[c] * inv_count : 0.f;
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
-          const float xc = __fsub_rn(xv[t], mean);
-          const float yv = __fmaf_rn(xc, sc, sh);
-          const float gy = yv > 0.f ? gv[t] : 0.f;
-          g[t] = sc * (gy - mg - xc * invstd * mgx);
+          const float gy = bn_preact(xv[t], mean, sc, sh) > 0.f ? gv[t] : 0.f;
+          g[t] = sc * (gy - mg - __fsub_rn(xv[t], mean) * invstd * mgx);
         }
       }
 #pragma unroll
@@ -204,48 +199,6 @@ __global__ void __launch_bounds__(256) bn_relu_bwd_apply_kernel(const T* __restr
       g_pm[((size_t)b * M + q0 + ql) * Cp + cb + cl] = s_tile[ql][cl];
     }
     __syncthreads();
-  }
-}
-
-// dgamma[c] = sum gy*xhat, dbeta[c] = sum gy from the partials: reuse the generic fixed-order reduction
-__global__ void __launch_bounds__(1024) bn_reduce2_kernel(const float* __restrict__ partial, int ntiles, int C,
-                                                          float* __restrict__ dgb /*(2,C): dgamma, dbeta*/) {
-  __shared__ double s1[32][33], s2[32][33];
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  const int c = blockIdx.x * 32 + tx;
-  double a1 = 0.0, a2 = 0.0;
-  if (c < C) {
-    double b1 = 0.0, b2 = 0.0, c1 = 0.0, c2 = 0.0, d1 = 0.0, d2 = 0.0;
-    int t = ty;
-    for (; t + 96 < ntiles; t += 128) {
-      a1 += (double)partial[((size_t)t * 2 + 0) * C + c];
-      a2 += (double)partial[((size_t)t * 2 + 1) * C + c];
-      b1 += (double)partial[((size_t)(t + 32) * 2 + 0) * C + c];
-      b2 += (double)partial[((size_t)(t + 32) * 2 + 1) * C + c];
-      c1 += (double)partial[((size_t)(t + 64) * 2 + 0) * C + c];
-      c2 += (double)partial[((size_t)(t + 64) * 2 + 1) * C + c];
-      d1 += (double)partial[((size_t)(t + 96) * 2 + 0) * C + c];
-      d2 += (double)partial[((size_t)(t + 96) * 2 + 1) * C + c];
-    }
-    for (; t < ntiles; t += 32) {
-      a1 += (double)partial[((size_t)t * 2 + 0) * C + c];
-      a2 += (double)partial[((size_t)t * 2 + 1) * C + c];
-    }
-    a1 = (a1 + b1) + (c1 + d1);
-    a2 = (a2 + b2) + (c2 + d2);
-  }
-  s1[ty][tx] = a1;
-  s2[ty][tx] = a2;
-  __syncthreads();
-  if (ty == 0 && c < C) {
-    double sgy = 0.0, sgx = 0.0;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      sgy += s1[i][tx];
-      sgx += s2[i][tx];
-    }
-    dgb[c] = (float)sgx;      // dgamma
-    dgb[C + c] = (float)sgy;  // dbeta
   }
 }
 
@@ -296,7 +249,8 @@ extern "C" int cl3d_bn_relu_bwd(const void* grad_y, int dtype, const float* x, c
     using T = typename decltype(t)::type;
     const T* gy = static_cast<const T*>(grad_y);
     bn_relu_bwd_stats_kernel<T><<<ntiles, 256, 0, stream>>>(gy, x, save_stats, gamma, beta, C, M, partial); CL3D_LAUNCHED(1);
-    bn_reduce2_kernel<<<ceil_div(C, 32), 1024, 0, stream>>>(partial, ntiles, C, dgamma_dbeta); CL3D_LAUNCHED(1);
+    const int rc = cl3d_reduce_partials(partial, ntiles, 2 * C, dgamma_dbeta, stream_);  // (dgamma, dbeta)
+    if (rc) return rc;
     bn_relu_bwd_apply_kernel<T><<<ntiles, 256, 0, stream>>>(gy, x, save_stats, gamma, beta, dgamma_dbeta, C, Cp, M,
                                                             1.0f / (float)((long long)B * M), training, g_pm); CL3D_LAUNCHED(1);
     return check_launch("bn_relu_bwd kernels");

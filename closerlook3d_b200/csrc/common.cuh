@@ -144,6 +144,13 @@ __device__ __forceinline__ void store_bn_moments(float* partial, size_t tile, in
   p[3 * C] = q;
 }
 
+// BatchNorm pre-activation (x - mean) * sc + sh with sc = invstd * gamma, sh = beta, rounded exactly as written.  Every
+// ReLU forward and every backward that recomputes the ReLU decision takes it from here, so they agree bit for bit (the
+// backward cannot decide from the output: a 16-bit output may round a small positive value to zero).
+__device__ __forceinline__ float bn_preact(float x, float mean, float sc, float sh) {
+  return __fmaf_rn(__fsub_rn(x, mean), sc, sh);
+}
+
 // one tile row held one value per lane (queries q0 + lane, present where q < M; lane 0 always is), centred about its
 // fp32 mean (a centre at one of the values would make sum (x - c)^2 cancel when that value is an outlier, e.g. a
 // padded query); absent lanes count nothing

@@ -29,6 +29,7 @@
 //                           slot-0 entries, d/dT from the dense term and the arg-max entries) summed in list order
 //                           and stored once -- in eval mode too (no dense term there)
 #include <mutex>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -52,8 +53,6 @@ struct PwArgs {
   unsigned char* karg;       // (B,M,Cop) first arg-max slot
   float* partial;            // fwd: (ntiles,kBnRows,Cout) ; bwd sparse: (ntiles,3,Cout) dWp partials
   // backward only
-  const float* grad_out;     // unused, kept for the layout of this block: pwmlp_bwd_stats_kernel takes grad_out as
-  const float* out;          // a kernel argument, and nothing reads out
   const float* stats;        // (2,Cout) mean, invstd
   const float* gamma;        // (Cout)
   const float* dgb;          // (2,Cout): sum dz*yhat, sum dz
@@ -241,29 +240,10 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_fwd_kernel(const PwArgs a
   }
 }
 
-// out[b,o,q] = relu(sc*ysel + sh)
-template <typename T>
-__global__ void __launch_bounds__(256) pwmlp_out_kernel(const float* __restrict__ ysel, const float* __restrict__ stats,
-                                                        const float* __restrict__ gamma,
-                                                        const float* __restrict__ beta, int C, int M,
-                                                        T* __restrict__ out) {
-  const int row = blockIdx.x;
-  const int c = row % C;
-  const float mean = stats[c], sc = stats[C + c] * gamma[c], sh = beta[c];
-  const float* src = ysel + (size_t)row * M;
-  T* dst = out + (size_t)row * M;
-  for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < M; i += gridDim.y * blockDim.x) {
-    const float v = __fmaf_rn(__fsub_rn(src[i], mean), sc, sh);  // pwmlp_bwd_stats_kernel recomputes this
-    store_f32(dst + i, v > 0.f ? v : 0.f);
-  }
-}
-
 // =================================================================================================
 // backward
 // =================================================================================================
-// The ReLU decision is recomputed from ysel and the BatchNorm constants with pwmlp_out_kernel's expression, which gives
-// the forward's fp32 decision bit for bit (a 16-bit output can round a small positive value to zero, so it cannot
-// decide).
+// The ReLU decision is recomputed from ysel with bn_preact, as the forward (cl3d_bn_relu_fwd) made it.
 template <typename TG>
 __global__ void __launch_bounds__(256) pwmlp_bwd_stats_kernel(const TG* __restrict__ grad_out,
                                                               const float* __restrict__ ysel,
@@ -282,7 +262,7 @@ __global__ void __launch_bounds__(256) pwmlp_bwd_stats_kernel(const TG* __restri
     float dz = 0.f, dzy = 0.f, sc = 0.f;
     if (c < C && q < M) {
       const size_t o = ((size_t)b * C + c) * M + q;
-      const bool pass = __fmaf_rn(__fsub_rn(ysel[o], stats[c]), stats[C + c] * gamma[c], beta[c]) > 0.f;
+      const bool pass = bn_preact(ysel[o], stats[c], stats[C + c] * gamma[c], beta[c]) > 0.f;
       dz = pass ? load_f32(grad_out + o) : 0.f;
       dzy = dz * ((ysel[o] - stats[c]) * stats[C + c]);
       sc = stats[C + c] * gamma[c];
@@ -389,13 +369,19 @@ __global__ void __launch_bounds__(kPWWarps * 32) pwmlp_bwd_dense_kernel(const Pw
 // Layers wider than 4 * kPWQGroups channels split their channel groups over blockIdx.y (one slice per CTA).
 constexpr int kPWQPT = 8;        // queries per thread
 constexpr int kPWQGroups = 256;  // channel groups of 4 per CTA slice (= the block size when ny = 1)
+constexpr int kPWQThreads = 256;  // block size: nx channel groups x ny query lanes
+__host__ __device__ inline int pw_query_nx(int Cop) {
+  const int ngroups = Cop >> 2;
+  return ngroups < kPWQGroups ? ngroups : kPWQGroups;
+}
+
 // DET (deterministic mode): no reductions into grad_ab; da' is stored point-major in da_pm (B,M,Cop) and
 // pwmlp_bwd_gather_det_kernel builds every grad_ab row from the canonical lists.
 template <bool DET>
 __device__ __forceinline__ void pwmlp_bwd_query_body(const PwArgs& a, long long nqueries, float* __restrict__ da_pm) {
   extern __shared__ float s_dw[];  // [ny][3][Cop]
   const int ngroups = a.Cop >> 2;
-  const int nx = ngroups < kPWQGroups ? ngroups : kPWQGroups, ny = blockDim.x / nx;
+  const int nx = pw_query_nx(a.Cop), ny = blockDim.x / nx;
   const int x = blockIdx.y * nx + threadIdx.x % nx, y = threadIdx.x / nx;
   const bool active = x < ngroups;  // the last slice of a wide layer may be narrower than nx
   const int c4 = x * 4;
@@ -470,12 +456,12 @@ __device__ __forceinline__ void pwmlp_bwd_query_body(const PwArgs& a, long long 
   }
 }
 
-__global__ void __launch_bounds__(256) pwmlp_bwd_query_kernel(const PwArgs a, long long nqueries /* B*M */) {
+__global__ void __launch_bounds__(kPWQThreads) pwmlp_bwd_query_kernel(const PwArgs a, long long nqueries /* B*M */) {
   pwmlp_bwd_query_body<false>(a, nqueries, nullptr);
 }
 
-__global__ void __launch_bounds__(256) pwmlp_bwd_query_det_kernel(const PwArgs a, long long nqueries,
-                                                                  float* __restrict__ da_pm) {
+__global__ void __launch_bounds__(kPWQThreads) pwmlp_bwd_query_det_kernel(const PwArgs a, long long nqueries,
+                                                                          float* __restrict__ da_pm) {
   pwmlp_bwd_query_body<true>(a, nqueries, da_pm);
 }
 
@@ -622,47 +608,50 @@ __global__ void pwmlp_wgrad_kernel(const float* __restrict__ gwcat, const float*
   }
 }
 
-static int pw_ci(int Cop) {
-  int ci = ceil_div(Cop, 32);
-  return ci > kPWMaxCI ? kPWMaxCI : ci;
-}
-
-template <int CI>
-static int launch_pw_fwd(const PwArgs& a, cudaStream_t stream) {
-  const size_t smem = align_up((size_t)kPWWarps * a.K * 4, 16) + (size_t)32 * CI * (kPWTile + 1) * 4 +
-                      (size_t)kPWWarps * 4 * 32 * CI * 4;
-  static std::atomic<unsigned long long> seen{0};
-  allow_big_smem(pwmlp_fwd_kernel<CI>, seen);
-  dim3 grid(a.ntiles, ceil_div(a.Cop, 32 * CI));
-  pwmlp_fwd_kernel<CI><<<grid, kPWWarps * 32, smem, stream>>>(a);
-  CL3D_LAUNCHED(1);
-  return check_launch("pwmlp_fwd_kernel");
-}
-template <int CI>
-static int launch_pw_bwd(const PwArgs& a, int ntiles_n, int gx, cudaStream_t stream) {
-  PwArgs d = a;
-  d.ntiles = ntiles_n;
-  pwmlp_bwd_dense_kernel<CI><<<dim3(gx, ceil_div(a.Cop, 32 * CI)), kPWWarps * 32, 0, stream>>>(d);
-  CL3D_LAUNCHED(1);
-  return check_launch("pwmlp_bwd_dense_kernel");
-}
-
-template <int CI>
-static int launch_pw_bwd_det(const PwArgs& a, const float* da_pm, int ntiles_n, int gx, cudaStream_t stream) {
-  PwArgs d = a;
-  d.ntiles = ntiles_n;
-  pwmlp_bwd_gather_det_kernel<CI><<<dim3(gx, ceil_div(a.Cop, 32 * CI)), kPWWarps * 32, 0, stream>>>(d, da_pm);
-  CL3D_LAUNCHED(1);
-  return check_launch("pwmlp_bwd_gather_det_kernel");
+// Calls fn(std::integral_constant<int, CI>{}) with CI = the 32-channel chunks one CTA of the forward or of a
+// support-major pass covers (kPWMaxCI at most), and returns its result.
+template <typename F>
+static int with_pw_ci(int Cop, F&& fn) {
+  switch (ceil_div(Cop, 32)) {
+    case 1: return fn(std::integral_constant<int, 1>{});
+    case 2: return fn(std::integral_constant<int, 2>{});
+    case 3: return fn(std::integral_constant<int, 3>{});
+    default: return fn(std::integral_constant<int, kPWMaxCI>{});
+  }
 }
 
 static int pw_dense_grid(int ntiles_n) {
   int gx = persistent_grid_cap();
   return gx > ntiles_n ? ntiles_n : gx;
 }
-static int pw_query_grid(int B, int M, int Cop) {
-  const int ny = 256 / (Cop / 4 < kPWQGroups ? Cop / 4 : kPWQGroups);  // queries per CTA row (pwmlp_bwd_query_kernel)
-  return (int)(((long long)B * M + (long long)ny * kPWQPT - 1) / ((long long)ny * kPWQPT));
+
+// Query pass launch (pwmlp_bwd_query_kernel / _det_kernel): nx channel groups x ny query lanes, kPWQPT queries per
+// thread; grid.y slices the channel groups of layers wider than 4 * kPWQGroups; shared memory holds [ny][3][Cop].
+struct PwQueryLaunch {
+  dim3 grid, block;
+  size_t smem;
+};
+static PwQueryLaunch pw_query_launch(int B, int M, int Cop) {
+  const int nx = pw_query_nx(Cop), ny = kPWQThreads / nx;
+  const long long per_cta = (long long)ny * kPWQPT;
+  return {dim3((unsigned)(((long long)B * M + per_cta - 1) / per_cta), ceil_div(Cop / 4, nx)), dim3(ny * nx),
+          (size_t)ny * 3 * Cop * sizeof(float)};
+}
+
+// Backward scratch, parts 64-float aligned: [ partials | sc*dz (B,M,Cop) | d/da' (B,M,Cop), deterministic mode only ].
+// The partials are the statistics pass's (2 rows of Cout per query tile), then the query pass's d/dWp (3 rows per CTA).
+struct PwScratch {
+  size_t dzs, da, floats;  // offsets of sc*dz and d/da' (the partials start at 0); the size
+};
+static PwScratch pw_scratch(int B, int M, int Cout, int deterministic) {
+  const int Cop = padded_channels(Cout);
+  const size_t stats_rows = (size_t)B * ceil_div(M, kPWTile) * 2, wp_rows = (size_t)pw_query_launch(B, M, Cop).grid.x * 3;
+  const size_t pm = (size_t)B * M * Cop;
+  PwScratch s;
+  s.dzs = align_up((stats_rows > wp_rows ? stats_rows : wp_rows) * Cout, 64);
+  s.da = s.dzs + align_up(pm, 64);
+  s.floats = deterministic ? s.da + pm : s.dzs + pm;
+  return s;
 }
 
 }  // namespace cl3d
@@ -719,38 +708,21 @@ extern "C" int cl3d_pwmlp_fwd_stats(const float* ab_pm, const float* wp, const f
   a.B = B; a.N = N; a.M = M; a.K = K; a.Cout = Cout; a.Cop = padded_channels(Cout);
   a.inv_radius = 1.0f / radius;
   a.ntiles = B * ceil_div(M, kPWTile);
-  switch (pw_ci(a.Cop)) {
-    case 1: return launch_pw_fwd<1>(a, (cudaStream_t)stream_);
-    case 2: return launch_pw_fwd<2>(a, (cudaStream_t)stream_);
-    case 3: return launch_pw_fwd<3>(a, (cudaStream_t)stream_);
-    default: return launch_pw_fwd<4>(a, (cudaStream_t)stream_);
-  }
-}
-
-extern "C" int cl3d_pwmlp_fwd_out(const float* ysel, const float* save_stats, const float* gamma, const float* beta,
-                                  int B, int M, int Cout, void* out, int dtype, cl3d_stream_t stream_) {
-  CL3D_REQUIRE(ysel && save_stats && gamma && beta && out && B >= 0 && M >= 1 && Cout >= 1,
-               "cl3d_pwmlp_fwd_out: bad arguments");
-  CL3D_REQUIRE_DTYPE(dtype, "cl3d_pwmlp_fwd_out");
-  if (B == 0) return CL3D_OK;
-  int chunks = ceil_div(M, 1024);
-  chunks = chunks < 1 ? 1 : (chunks > 65535 ? 65535 : chunks);
-  return with_dtype(dtype, [&](auto t) {
-    using T = typename decltype(t)::type;
-    pwmlp_out_kernel<T><<<dim3(B * Cout, chunks), 256, 0, (cudaStream_t)stream_>>>(ysel, save_stats, gamma, beta, Cout, M,
-                                                                                   static_cast<T*>(out));
+  return with_pw_ci(a.Cop, [&](auto ci) {
+    constexpr int CI = decltype(ci)::value;
+    const size_t smem = align_up((size_t)kPWWarps * a.K * 4, 16) + (size_t)32 * CI * (kPWTile + 1) * 4 +
+                        (size_t)kPWWarps * 4 * 32 * CI * 4;
+    static std::atomic<unsigned long long> seen{0};
+    allow_big_smem(pwmlp_fwd_kernel<CI>, seen);
+    pwmlp_fwd_kernel<CI><<<dim3(a.ntiles, ceil_div(a.Cop, 32 * CI)), kPWWarps * 32, smem, (cudaStream_t)stream_>>>(a);
     CL3D_LAUNCHED(1);
-    return check_launch("pwmlp_out_kernel");
+    return check_launch("pwmlp_fwd_kernel");
   });
 }
 
 extern "C" size_t cl3d_pwmlp_bwd_scratch_floats(int B, int N, int M, int Cout, int deterministic) {
-  const int Cop = padded_channels(Cout);
   (void)N;
-  const size_t ntm = (size_t)B * ceil_div(M, kPWTile), gq = (size_t)pw_query_grid(B, M, Cop);
-  const size_t part = (ntm * 2 > gq * 3 ? ntm * 2 : gq * 3) * (size_t)Cout;
-  // deterministic: da' point-major (B*M*Cop) behind sc*dz
-  return part + (size_t)B * M * Cop * (deterministic ? 2 : 1) + 64 + (deterministic ? 64 : 0);
+  return pw_scratch(B, M, Cout, deterministic).floats;
 }
 
 // fork/join events of cl3d_pwmlp_bwd: a small per-device ring of event sets, so that several calls can be in
@@ -805,13 +777,12 @@ extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta
   const int ntn = B * ceil_div(N, kPWTile);
   const int gx = pw_dense_grid(ntn);
   const int Cop = padded_channels(Cout);
-  // scratch = [ partials (max(ntiles*2, gx*3) * Cout) | dzs_pm (B*M*Cop) ]
-  const int gqy = pw_query_grid(B, M, Cop);
-  const size_t part = ((size_t)ntiles * 2 > (size_t)gqy * 3 ? (size_t)ntiles * 2 : (size_t)gqy * 3) * (size_t)Cout;
+  const PwQueryLaunch ql = pw_query_launch(B, M, Cop);
+  const PwScratch sl = pw_scratch(B, M, Cout, deterministic);
   float* partial = scratch;
-  float* dzs_pm = scratch + ((part + 63) / 64) * 64;
+  float* dzs_pm = scratch + sl.dzs;
+  float* da_pm = scratch + sl.da;  // deterministic mode only
   const size_t smem_s = (size_t)kPWTile * (Cop + 1) * sizeof(float);
-  float* da_pm = dzs_pm + (((size_t)B * M * Cop + 63) / 64) * 64;  // deterministic mode only
   if (forked) {
     cudaEventRecord(ev->start, stream);
     cudaStreamWaitEvent(side, ev->start, 0);
@@ -849,39 +820,35 @@ extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta
   // eval mode (frozen BatchNorm): the batch-statistics terms c1, c2 vanish (inv_count = 0 zeroes them in the query
   // pass) and the dense support-major pass would add exact zeros, so it is not launched
   a.inv_count = training ? 1.0f / (float)((double)B * M * K) : 0.f;
-  a.ntiles = ntiles;
+  a.ntiles = ntn;  // the support-major passes walk tiles of support points
   if (deterministic) {
-    const int nx = Cop / 4 < kPWQGroups ? Cop / 4 : kPWQGroups, ny = 256 / nx;
-    pwmlp_bwd_query_det_kernel<<<dim3(gqy, ceil_div(Cop / 4, nx)), ny * nx, (size_t)ny * 3 * Cop * sizeof(float),
-                                 stream>>>(a, (long long)B * M, da_pm);
+    pwmlp_bwd_query_det_kernel<<<ql.grid, ql.block, ql.smem, stream>>>(a, (long long)B * M, da_pm);
     CL3D_LAUNCHED(1);
     rc = check_launch("pwmlp_bwd_query_det_kernel");
     if (rc) return rc;
-    rc = cl3d_reduce_partials(partial, gqy, 3 * Cout, grad_wp, stream_);
+    rc = cl3d_reduce_partials(partial, (int)ql.grid.x, 3 * Cout, grad_wp, stream_);
     if (rc) return rc;
-    switch (pw_ci(Cop)) {
-      case 1: return launch_pw_bwd_det<1>(a, da_pm, ntn, gx, stream);
-      case 2: return launch_pw_bwd_det<2>(a, da_pm, ntn, gx, stream);
-      case 3: return launch_pw_bwd_det<3>(a, da_pm, ntn, gx, stream);
-      default: return launch_pw_bwd_det<4>(a, da_pm, ntn, gx, stream);
-    }
+    return with_pw_ci(Cop, [&](auto ci) {
+      constexpr int CI = decltype(ci)::value;
+      pwmlp_bwd_gather_det_kernel<CI><<<dim3(gx, ceil_div(Cop, 32 * CI)), kPWWarps * 32, 0, stream>>>(a, da_pm);
+      CL3D_LAUNCHED(1);
+      return check_launch("pwmlp_bwd_gather_det_kernel");
+    });
   }
   if (training) {
-    switch (pw_ci(Cop)) {
-      case 1: rc = launch_pw_bwd<1>(a, ntn, gx, stream); break;
-      case 2: rc = launch_pw_bwd<2>(a, ntn, gx, stream); break;
-      case 3: rc = launch_pw_bwd<3>(a, ntn, gx, stream); break;
-      default: rc = launch_pw_bwd<4>(a, ntn, gx, stream); break;
-    }
+    rc = with_pw_ci(Cop, [&](auto ci) {
+      constexpr int CI = decltype(ci)::value;
+      pwmlp_bwd_dense_kernel<CI><<<dim3(gx, ceil_div(Cop, 32 * CI)), kPWWarps * 32, 0, stream>>>(a);
+      CL3D_LAUNCHED(1);
+      return check_launch("pwmlp_bwd_dense_kernel");
+    });
     if (rc) return rc;
   }
-  const int nx = Cop / 4 < kPWQGroups ? Cop / 4 : kPWQGroups, ny = 256 / nx;
-  pwmlp_bwd_query_kernel<<<dim3(gqy, ceil_div(Cop / 4, nx)), ny * nx, (size_t)ny * 3 * Cop * sizeof(float), side>>>(
-      a, (long long)B * M);
+  pwmlp_bwd_query_kernel<<<ql.grid, ql.block, ql.smem, side>>>(a, (long long)B * M);
   CL3D_LAUNCHED(1);
   rc = check_launch("pwmlp_bwd_query_kernel");
   if (rc) return rc;
-  rc = cl3d_reduce_partials(partial, gqy, 3 * Cout, grad_wp, (cl3d_stream_t)side);
+  rc = cl3d_reduce_partials(partial, (int)ql.grid.x, 3 * Cout, grad_wp, (cl3d_stream_t)side);
   if (forked) {
     cudaEventRecord(ev->joined, side);
     cudaStreamWaitEvent(stream, ev->joined, 0);

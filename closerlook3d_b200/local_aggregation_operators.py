@@ -41,20 +41,14 @@ class _FusedAggBNReLU(Function):
         B, C, N = features.shape
         M = query_xyz.shape[1]
         feat_pm = ops.to_point_major(features)   # overlaps the neighbour search running on the side stream
-        training = bn.training or (bn.running_mean is None)
         arg = None
         if spec.reduction == ops.REDUCE["max"]:   # winning slot per (query, channel), read again by the backward
             arg = torch.empty(B, M, feat_pm.shape[2], dtype=torch.uint8, device=features.device)
         nl.wait()
         agg, partial = ops.agg_fwd(spec.family, spec.reduction, feat_pm, query_xyz, support_xyz, nl.idx, nl.ncount,
                                    p0, p1, C, spec.radius, spec.normalize, spec.shared, spec.nkp, spec.extent,
-                                   spec.influence, want_bn_partial=training, arg=arg)
-        momentum = bn.momentum if bn.momentum is not None else 0.0
-        if training and bn.running_mean is not None:
-            bn.num_batches_tracked.add_(1)
-            if bn.momentum is None:  # cumulative moving average, as nn.BatchNorm1d
-                momentum = 1.0 / float(bn.num_batches_tracked)
-        stats = ops.bn_finalize(partial, C, B * M, bn.eps, momentum, training, bn.running_mean, bn.running_var)
+                                   spec.influence, want_bn_partial=bn.training or bn.running_mean is None, arg=arg)
+        stats, training = ops.bn_batch_stats(bn, partial, C, B * M)
         out = ops.bn_relu_fwd(agg, stats, bn_weight, bn_bias, dtype=features.dtype)
         if any(ctx.needs_input_grad):
             nl.prefetch_csr(all_slots=False)      # transposed lists for the backward, built behind the forward

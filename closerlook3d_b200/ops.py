@@ -293,6 +293,19 @@ def bn_finalize(bn_partial, C, count, eps, momentum, training, running_mean, run
     return stats
 
 
+def bn_batch_stats(bn, partial, C, count):
+    """The BatchNorm statistics a fused forward normalises with, as nn.BatchNorm in `bn`'s mode: batch statistics
+    (updating the running ones, momentum=None as a cumulative average) when training or when there are no running
+    statistics, else the running ones.  -> (save_stats (2,C): mean, invstd; training)"""
+    training = bn.training or bn.running_mean is None
+    momentum = bn.momentum if bn.momentum is not None else 0.0
+    if training and bn.running_mean is not None:
+        bn.num_batches_tracked.add_(1)
+        if bn.momentum is None:
+            momentum = 1.0 / float(bn.num_batches_tracked)
+    return bn_finalize(partial, C, count, bn.eps, momentum, training, bn.running_mean, bn.running_var), training
+
+
 @_on_device
 def bn_relu_fwd(x, stats, gamma, beta, dtype=F32):
     """x (B,C,M) fp32 -> y in `dtype`"""
@@ -388,15 +401,6 @@ def pwmlp_fwd_stats(ab_pm, wp, sgn, query_xyz, support_xyz, idx, Cout, radius):
                                  float(radius), ptr(ysel), ptr(aq), ptr(sq), ptr(karg), ptr(partial), stream_ptr()),
           "cl3d_pwmlp_fwd_stats")
     return ysel, aq, sq, karg, partial
-
-
-@_on_device
-def pwmlp_fwd_out(ysel, stats, gamma, beta, dtype=F32):
-    B, Cout, M = ysel.shape
-    out = torch.empty(B, Cout, M, dtype=dtype, device=ysel.device)
-    check(_lib.lib().cl3d_pwmlp_fwd_out(ptr(ysel), ptr(stats), ptr(gamma), ptr(beta), B, M, Cout, ptr(out),
-                                        DTYPE_CODE[dtype], stream_ptr()), "cl3d_pwmlp_fwd_out")
-    return out
 
 
 @_on_device

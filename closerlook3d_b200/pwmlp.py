@@ -28,18 +28,11 @@ class _FusedPointWiseMLP(Function):
         # AB[p][n] = sum_c fa[p][c] * wcat[n][c]   (both row-padded to Cpa with zeros -> k runs over Cpa)
         ab_pm = ops.sgemm(fa_pm, Cpa, 1, wcat, 1, Cpa, B * N, 2 * Cop, Cpa).view(B, N, 2 * Cop)
         nl.wait()                                   # the search ran on the side stream, overlapping the product
-        training = bn.training or (bn.running_mean is None)
-        if any(ctx.needs_input_grad) and (training or ops.deterministic_mode()):
+        if any(ctx.needs_input_grad) and (bn.training or bn.running_mean is None or ops.deterministic_mode()):
             nl.prefetch_csr(all_slots=True)         # lists for the backward, built behind the forward kernels
         ysel, aq, sq, karg, partial = ops.pwmlp_fwd_stats(ab_pm, wp, sgn, query_xyz, support_xyz, nl.idx, Cout, radius)
-        momentum = bn.momentum if bn.momentum is not None else 0.0
-        if training and bn.running_mean is not None:
-            bn.num_batches_tracked.add_(1)
-            if bn.momentum is None:
-                momentum = 1.0 / float(bn.num_batches_tracked)
-        stats = ops.bn_finalize(partial, Cout, B * M * K, bn.eps, momentum, training, bn.running_mean,
-                                bn.running_var)
-        out = ops.pwmlp_fwd_out(ysel, stats, bn_weight, bn_bias, dtype=features.dtype)
+        stats, training = ops.bn_batch_stats(bn, partial, Cout, B * M * K)
+        out = ops.bn_relu_fwd(ysel, stats, bn_weight, bn_bias, dtype=features.dtype)
         ctx.nl, ctx.radius, ctx.training, ctx.dims = nl, radius, training, (B, C, N, M, K, Cout, Cop, Cpa)
         ctx.dtype = features.dtype
         # the backward recomputes the ReLU decision from ysel and the BatchNorm constants, not from `out`

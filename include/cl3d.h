@@ -225,8 +225,8 @@ int cl3d_reduce_partials(const float* partial, int ntiles, int P, float* out, cl
  *                centre near the tile's values), sum (x - c), sum (x - c)^2.  The tiles are merged in
  *                double, so a channel whose mean dwarfs its spread keeps its variance.
  *   bn_relu_fwd: y = relu((x-mean)*invstd*gamma + beta); in eval mode pass stats made from running stats.
- *   bn_relu_bwd_stats / bn_relu_bwd_apply: two-phase backward; apply writes d(loss)/d(agg) POINT-MAJOR
- *                (B,M,Cp) ready for cl3d_agg_bwd, and dgamma/dbeta.
+ *   bn_relu_bwd: per-tile partial rows (sum gy*xhat, sum gy) reduced as cl3d_reduce_partials into dgamma_dbeta, then
+ *                the apply pass writes d(loss)/d(agg) POINT-MAJOR (B,M,Cp) ready for cl3d_agg_bwd.
  *   y written / grad_y read in `dtype`; x, the statistics, partials, dgamma_dbeta and g_pm fp32.
  * ---------------------------------------------------------------------------------------------- */
 #define CL3D_BN_PARTIAL_ROWS 4
@@ -269,7 +269,8 @@ int cl3d_sgemm_algo(const float* a, long long sa_m, long long sa_k, const float*
  * fwd_stats : ysel (B,Cout,M) selected extremum of y; aq, sq (B,M,Cop) a' and sum_k bv; karg (B,M,Cop) uint8
  *             first arg-max slot (K <= 255); bn_partial (cl3d_agg_num_tiles(B,M), CL3D_BN_PARTIAL_ROWS, Cout) -> cl3d_bn_finalize
  *             with count = B*M*K.
- * fwd_out   : out (B,Cout,M) = relu(sc*ysel + sh), in `dtype`.
+ * output    : out (B,Cout,M) = relu(sc*ysel + sh) in `dtype` is cl3d_bn_relu_fwd(ysel, save_stats, gamma, beta, B, Cout,
+ *             M, out, dtype, stream).
  * bwd       : grad_out (B,Cout,M) in `dtype`.  The ReLU decision is recomputed from ysel, save_stats, gamma and beta
  *             with the forward's expression (bit-identical to the forward's fp32 decision; a 16-bit output may have
  *             rounded a small positive value to zero, so the stored output cannot decide).
@@ -298,8 +299,6 @@ int cl3d_pwmlp_fwd_stats(const float* ab_pm, const float* wp, const float* sgn, 
                          const float* support_xyz, const int* idx, int B, int N, int M, int K, int Cout,
                          float radius, float* ysel,
                          float* aq, float* sq, unsigned char* karg, float* bn_partial, cl3d_stream_t stream);
-int cl3d_pwmlp_fwd_out(const float* ysel, const float* save_stats, const float* gamma, const float* beta,
-                       int B, int M, int Cout, void* out, int dtype, cl3d_stream_t stream);
 int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta, const float* ab_pm, const float* wp,
                    const float* sgn, const float* query_xyz, const float* support_xyz, const int* idx,
                    const int* csr_off, const int* csr_ent, const float* ysel, const float* aq, const float* sq,

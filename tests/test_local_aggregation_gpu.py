@@ -217,8 +217,9 @@ def _declared_functions():
 @pytest.mark.parametrize("la_type,over,entries", [
     ("pseudo_grid", dict(), {"cl3d_to_point_major", "cl3d_agg_fwd", "cl3d_agg_bwd", "cl3d_bn_relu_fwd",
                              "cl3d_bn_relu_bwd"}),
-    ("pointwisemlp", PW, {"cl3d_sgemm_algo", "cl3d_pwmlp_fwd_stats", "cl3d_pwmlp_fwd_out", "cl3d_pwmlp_bwd",
-                          "cl3d_to_channel_major"}),
+    # the output is cl3d_bn_relu_fwd over the selected extremum
+    pytest.param("pointwisemlp", PW, {"cl3d_sgemm_algo", "cl3d_pwmlp_fwd_stats", "cl3d_bn_relu_fwd", "cl3d_pwmlp_bwd",
+                                      "cl3d_to_channel_major"}, id="pointwisemlp-output-bn_relu_fwd"),
 ])
 def test_profiler_records_declared_entry_points(cuda, la_type, over, entries):
     # bench.py's kernel model and tools/bench_pg.py look the profiler's records up by the names include/cl3d.h declares

@@ -11,9 +11,9 @@ MAP = [("gemm_tf32x3", "cl3d_sgemm_algo"), ("sgemm", "cl3d_sgemm_algo"), ("split
        ("pg2_kernel<(bool)0", "cl3d_agg_fwd"), ("pg2_kernel<(bool)1", "cl3d_agg_bwd"), ("pg2_kernel<0", "cl3d_agg_fwd"),
        ("pg2_kernel<1", "cl3d_agg_bwd"), ("pg3_bwd_kernel", "cl3d_agg_bwd"), ("pg3_fwd_kernel", "cl3d_agg_fwd"),
        ("aggmax_fwd", "cl3d_agg_fwd"), ("aggmax_bwd", "cl3d_agg_bwd"), ("nearest_query", "cl3d_nearest_query"),
-       ("pwmlp_fwd_kernel", "cl3d_pwmlp_fwd_stats"), ("pwmlp_out", "cl3d_pwmlp_fwd_out"), ("pwmlp_bwd", "cl3d_pwmlp_bwd"),
+       ("pwmlp_fwd_kernel", "cl3d_pwmlp_fwd_stats"), ("pwmlp_bwd", "cl3d_pwmlp_bwd"),
        ("agg_fwd", "cl3d_agg_fwd"), ("sincos_fwd", "cl3d_agg_fwd"), ("agg_bwd", "cl3d_agg_bwd"), ("sincos_bwd", "cl3d_agg_bwd"),
-       ("bn_relu_fwd", "cl3d_bn_relu_fwd"), ("bn_relu_bwd", "cl3d_bn_relu_bwd"), ("bn_reduce2", "cl3d_bn_relu_bwd"),
+       ("bn_relu_fwd", "cl3d_bn_relu_fwd"), ("bn_relu_bwd", "cl3d_bn_relu_bwd"),
        ("bn_finalize", "cl3d_bn_finalize"), ("to_point_major_aug", "cl3d_to_point_major_aug"),
        ("to_point_major", "cl3d_to_point_major"), ("pwmlp_prep", "cl3d_pwmlp_prep_weights"),
        ("pwmlp_wgrad", "cl3d_pwmlp_weight_grad"), ("reduce_partials", "cl3d_reduce_partials"),
