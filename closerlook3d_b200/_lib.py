@@ -50,6 +50,10 @@ SIGNATURES = {
     "cl3d_bn_finalize": (_i, [_vp, _i, _i, _ll, _f, _f, _i, _vp, _vp, _vp, _vp]),
     "cl3d_bn_relu_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp]),
     "cl3d_bn_relu_bwd": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "cl3d_bn_relu_bwd_stats": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "cl3d_bn_relu_bwd_apply": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "cl3d_bn_rank_moments": (_i, [_vp, _i, _i, _ll, _vp, _vp]),
+    "cl3d_bn_finalize_ranks": (_i, [_vp, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp]),
     "cl3d_sgemm_workspace_bytes": (_sz, [_i, _i, _i]),
     "cl3d_sgemm_algo": (_i, [_vp, _ll, _ll, _vp, _ll, _ll, _i, _i, _i, _vp, _ll, _i, _vp, _sz, _i, _vp]),
     "cl3d_pwmlp_prep_weights": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
@@ -58,6 +62,8 @@ SIGNATURES = {
     "cl3d_pwmlp_fwd_stats": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp]),
     "cl3d_pwmlp_bwd_scratch_floats": (_sz, [_i, _i, _i, _i, _i]),
     "cl3d_pwmlp_bwd": (_i, [_vp, _i] + [_vp] * 15 + [_i, _i, _i, _i, _i, _f, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "cl3d_pwmlp_bwd_stats": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "cl3d_pwmlp_bwd_apply": (_i, [_vp, _i] + [_vp] * 15 + [_i, _i, _i, _i, _i, _f, _i, _i] + [_vp] * 7),
     "cl3d_mhead_save_floats": (_sz, [_i, _i]),
     "cl3d_mhead_fwd_workspace_bytes": (_sz, [_vp, _i, _i]),
     "cl3d_mhead_bwd_workspace_bytes": (_sz, [_vp, _i, _i]),

@@ -13,27 +13,24 @@
 
 namespace cl3d {
 
-// one tile's moments (store_bn_moments) added to the sums of (x - shift) and (x - shift)^2: with g = centre - shift,
+// one tile's moments (store_bn_moments), or one rank's record (cl3d_bn_rank_moments), added to the sums of (x - shift)
+// and (x - shift)^2: with g = centre - shift,
 //   sum (x - shift) = d + n g,   sum (x - shift)^2 = q + 2 g d + n g^2
-__device__ __forceinline__ void bn_tile_add(const float* __restrict__ p, int C, double shift, double& a1, double& a2) {
+template <typename T>
+__device__ __forceinline__ void bn_tile_add(const T* __restrict__ p, int C, double shift, double& a1, double& a2) {
   const double n = p[0], g = (double)p[C] - shift, d = p[2 * C], q = p[3 * C];
   a1 += fma(n, g, d);
   a2 += fma(g, fma(n, g, 2.0 * d), q);
 }
 
-// mean / invstd from the per-tile moments; running-stat update as nn.BatchNorm1d (unbiased variance).
-// The tiles are merged in double about one shift per channel, tile 0's centre (a value of the channel, so the sums
-// are of spread-sized terms and the variance never cancels against the mean), in a fixed order: deterministic.
-// One CTA = 8 channels (one 32-byte sector of a partial row) x 128 tile slices: C/8 CTAs, so the whole partial
-// array is in flight at once (the kernel sits on the forward's critical path and is pure load latency).
-__global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restrict__ partial, int ntiles, int C,
-                                                           double count, float eps, float momentum, int training,
-                                                           float* __restrict__ running_mean,
-                                                           float* __restrict__ running_var,
-                                                           float* __restrict__ save_stats) {
-  __shared__ double s1[128][9], s2[128][9];
-  const int tx = threadIdx.x & 7, ty = threadIdx.x >> 3;
-  const int c = blockIdx.x * 8 + tx;
+// The tiles of a forward's partials merged in double about one shift per channel, tile 0's centre (a value of the
+// channel, so the sums are of spread-sized terms and the variance never cancels against the mean), in a fixed order:
+// deterministic.  One CTA of 1024 threads = 8 channels (one 32-byte sector of a partial row) x 128 tile slices, so the
+// whole partial array is in flight at once (pure load latency).  Every thread calls it with tx = threadIdx.x & 7,
+// ty = threadIdx.x >> 3 and c = blockIdx.x * 8 + tx; it returns the shift, and s1[0][tx], s2[0][tx] then hold channel
+// c's sum (x - shift) and sum (x - shift)^2 (all zero when training = 0 or c >= C).
+__device__ __forceinline__ double bn_merge_tiles(const float* __restrict__ partial, int ntiles, int C, int training,
+                                                 int tx, int ty, int c, double (&s1)[128][9], double (&s2)[128][9]) {
   const size_t ts = (size_t)kBnRows * C;  // floats per tile
   const double shift = training && c < C ? (double)partial[C + c] : 0.0;
   double a1 = 0.0, a2 = 0.0;
@@ -62,24 +59,97 @@ __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restri
     }
     __syncthreads();
   }
+  return shift;
+}
+
+// batch mean / invstd of channel c from its merged sums about `shift`; running-stat update as nn.BatchNorm1d
+// (unbiased variance over `count`)
+__device__ __forceinline__ void bn_store_batch_stats(int c, int C, double count, double shift, double sum1, double sum2,
+                                                     float eps, float momentum, float* __restrict__ running_mean,
+                                                     float* __restrict__ running_var, float* __restrict__ save_stats) {
+  const double dm = sum1 / count;  // mean - shift
+  const double mean = shift + dm;
+  double var = sum2 / count - dm * dm;
+  if (var < 0.0) var = 0.0;
+  save_stats[c] = (float)mean;
+  save_stats[C + c] = (float)(1.0 / sqrt(var + (double)eps));
+  if (running_mean && running_var) {
+    const double unbiased = count > 1.0 ? var * count / (count - 1.0) : var;
+    running_mean[c] = (float)((1.0 - (double)momentum) * (double)running_mean[c] + (double)momentum * mean);
+    running_var[c] = (float)((1.0 - (double)momentum) * (double)running_var[c] + (double)momentum * unbiased);
+  }
+}
+
+// mean / invstd from the per-tile moments (training) or from the running statistics (eval)
+__global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restrict__ partial, int ntiles, int C,
+                                                           double count, float eps, float momentum, int training,
+                                                           float* __restrict__ running_mean,
+                                                           float* __restrict__ running_var,
+                                                           float* __restrict__ save_stats) {
+  __shared__ double s1[128][9], s2[128][9];
+  const int tx = threadIdx.x & 7, ty = threadIdx.x >> 3;
+  const int c = blockIdx.x * 8 + tx;
+  const double shift = bn_merge_tiles(partial, ntiles, C, training, tx, ty, c, s1, s2);
   if (ty == 0 && c < C) {
     if (training) {
-      const double dm = s1[0][tx] / count;  // mean - shift
-      const double mean = shift + dm;
-      double var = s2[0][tx] / count - dm * dm;
-      if (var < 0.0) var = 0.0;
-      save_stats[c] = (float)mean;
-      save_stats[C + c] = (float)(1.0 / sqrt(var + (double)eps));
-      if (running_mean && running_var) {
-        const double unbiased = count > 1.0 ? var * count / (count - 1.0) : var;
-        running_mean[c] = (float)((1.0 - (double)momentum) * (double)running_mean[c] + (double)momentum * mean);
-        running_var[c] = (float)((1.0 - (double)momentum) * (double)running_var[c] + (double)momentum * unbiased);
-      }
+      bn_store_batch_stats(c, C, count, shift, s1[0][tx], s2[0][tx], eps, momentum, running_mean, running_var,
+                           save_stats);
     } else {
       save_stats[c] = running_mean[c];
       save_stats[C + c] = 1.0f / sqrtf(running_var[c] + eps);
     }
   }
+}
+
+// one rank's record (4,C) float64 for the cross-rank merge: count, centre (tile 0's), sum (x - centre),
+// sum (x - centre)^2 -- the same merge as bn_finalize_kernel, stopped before the division
+__global__ void __launch_bounds__(1024) bn_rank_moments_kernel(const float* __restrict__ partial, int ntiles, int C,
+                                                               double count, double* __restrict__ record) {
+  __shared__ double s1[128][9], s2[128][9];
+  const int tx = threadIdx.x & 7, ty = threadIdx.x >> 3;
+  const int c = blockIdx.x * 8 + tx;
+  const double shift = bn_merge_tiles(partial, ntiles, C, 1, tx, ty, c, s1, s2);
+  if (ty == 0 && c < C) {
+    record[c] = count;
+    record[C + c] = shift;
+    record[2 * C + c] = s1[0][tx];
+    record[3 * C + c] = s2[0][tx];
+  }
+}
+
+// the W ranks' records (W,4,C) merged in rank order about rank 0's centre (bn_tile_add: every rank computes the same
+// bits); the global count is their sum, written to *count_out for the backward
+__global__ void __launch_bounds__(128) bn_finalize_ranks_kernel(const double* __restrict__ records, int W, int C,
+                                                                float eps, float momentum,
+                                                                float* __restrict__ running_mean,
+                                                                float* __restrict__ running_var,
+                                                                float* __restrict__ save_stats,
+                                                                double* __restrict__ count_out) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const double shift = records[C + c];
+  double a1 = 0.0, a2 = 0.0, count = 0.0;
+  for (int r = 0; r < W; ++r) {
+    const double* p = records + (size_t)r * 4 * C + c;
+    bn_tile_add(p, C, shift, a1, a2);
+    count += p[0];
+  }
+  if (c == 0) *count_out = count;
+  bn_store_batch_stats(c, C, count, shift, a1, a2, eps, momentum, running_mean, running_var, save_stats);
+}
+
+// out = sums * (1 / count): the batch-statistic means of the BatchNorm backward over a count held on the device, so
+// that an apply pass taking a host scalar inv_count can run with inv_count = 1
+__global__ void __launch_bounds__(256) bn_mean_terms_kernel(const float* __restrict__ sums, int n,
+                                                            const double* __restrict__ count, float* __restrict__ out) {
+  const float inv = 1.0f / (float)*count;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = sums[i] * inv;
+}
+
+int bn_mean_terms(const float* sums, int n, const double* count, float* out, cudaStream_t stream) {
+  bn_mean_terms_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(sums, n, count, out);
+  CL3D_LAUNCHED(1);
+  return check_launch("bn_mean_terms_kernel");
 }
 
 // y = relu((x - mean) * invstd * gamma + beta), channel-major, float4 along M when aligned
@@ -234,25 +304,79 @@ extern "C" int cl3d_bn_relu_fwd(const float* x, const float* save_stats, const f
   });
 }
 
+extern "C" int cl3d_bn_rank_moments(const float* bn_partial, int ntiles, int C, long long count, double* record,
+                                    cl3d_stream_t stream_) {
+  CL3D_REQUIRE(bn_partial && record && ntiles >= 1 && C >= 1 && count >= 1, "cl3d_bn_rank_moments: bad arguments");
+  bn_rank_moments_kernel<<<ceil_div(C, 8), 1024, 0, (cudaStream_t)stream_>>>(bn_partial, ntiles, C, (double)count,
+                                                                             record);
+  CL3D_LAUNCHED(1);
+  return check_launch("bn_rank_moments_kernel");
+}
+
+extern "C" int cl3d_bn_finalize_ranks(const double* records, int W, int C, float eps, float momentum,
+                                      float* running_mean, float* running_var, float* save_stats, double* count,
+                                      cl3d_stream_t stream_) {
+  CL3D_REQUIRE(records && save_stats && count && W >= 1 && C >= 1, "cl3d_bn_finalize_ranks: bad arguments");
+  bn_finalize_ranks_kernel<<<ceil_div(C, 128), 128, 0, (cudaStream_t)stream_>>>(records, W, C, eps, momentum,
+                                                                                running_mean, running_var, save_stats,
+                                                                                count);
+  CL3D_LAUNCHED(1);
+  return check_launch("bn_finalize_ranks_kernel");
+}
+
+extern "C" int cl3d_bn_relu_bwd_stats(const void* grad_y, int dtype, const float* x, const float* save_stats,
+                                      const float* gamma, const float* beta, int B, int C, int M, float* partial,
+                                      float* dgamma_dbeta, cl3d_stream_t stream_) {
+  CL3D_REQUIRE(grad_y && x && save_stats && gamma && beta && partial && dgamma_dbeta,
+               "cl3d_bn_relu_bwd_stats: null pointer");
+  CL3D_REQUIRE(B >= 0 && C >= 1 && M >= 1, "cl3d_bn_relu_bwd_stats: bad sizes");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_bn_relu_bwd_stats");
+  if (B == 0) return CL3D_OK;
+  const int ntiles = B * ceil_div(M, kBwdTile);  // <= cl3d_agg_num_tiles(B, M): the caller's partial buffer fits
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    bn_relu_bwd_stats_kernel<T><<<ntiles, 256, 0, (cudaStream_t)stream_>>>(static_cast<const T*>(grad_y), x, save_stats,
+                                                                           gamma, beta, C, M, partial);
+    CL3D_LAUNCHED(1);
+    return cl3d_reduce_partials(partial, ntiles, 2 * C, dgamma_dbeta, stream_);  // (dgamma, dbeta)
+  });
+}
+
+extern "C" int cl3d_bn_relu_bwd_apply(const void* grad_y, int dtype, const float* x, const float* save_stats,
+                                      const float* gamma, const float* beta, int B, int C, int M, int training,
+                                      const float* dgb_sums, const double* count, float* work, float* g_pm,
+                                      cl3d_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  CL3D_REQUIRE(grad_y && x && save_stats && gamma && beta && dgb_sums && g_pm && (!count || work),
+               "cl3d_bn_relu_bwd_apply: null pointer");
+  CL3D_REQUIRE(B >= 0 && C >= 1 && M >= 1, "cl3d_bn_relu_bwd_apply: bad sizes");
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_bn_relu_bwd_apply");
+  if (B == 0) return CL3D_OK;
+  const int ntiles = B * ceil_div(M, kBwdTile);
+  const int Cp = padded_channels(C);
+  float inv_count = 1.0f / (float)((long long)B * M);
+  const float* dgb = dgb_sums;
+  if (count && training) {  // the means over the device-held count, then the same apply pass with inv_count = 1
+    const int rc = bn_mean_terms(dgb_sums, 2 * C, count, work, stream);
+    if (rc) return rc;
+    dgb = work;
+    inv_count = 1.0f;
+  }
+  return with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    bn_relu_bwd_apply_kernel<T><<<ntiles, 256, 0, stream>>>(static_cast<const T*>(grad_y), x, save_stats, gamma, beta,
+                                                            dgb, C, Cp, M, inv_count, training, g_pm);
+    CL3D_LAUNCHED(1);
+    return check_launch("bn_relu_bwd kernels");
+  });
+}
+
 extern "C" int cl3d_bn_relu_bwd(const void* grad_y, int dtype, const float* x, const float* save_stats,
                                 const float* gamma, const float* beta, int B, int C, int M, int training,
                                 float* partial, float* dgamma_dbeta, float* g_pm, cl3d_stream_t stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
-  CL3D_REQUIRE(grad_y && x && save_stats && gamma && beta && partial && dgamma_dbeta && g_pm,
-               "cl3d_bn_relu_bwd: null pointer");
-  CL3D_REQUIRE(B >= 0 && C >= 1 && M >= 1, "cl3d_bn_relu_bwd: bad sizes");
-  CL3D_REQUIRE_DTYPE(dtype, "cl3d_bn_relu_bwd");
-  if (B == 0) return CL3D_OK;
-  const int ntiles = B * ceil_div(M, kBwdTile);  // <= cl3d_agg_num_tiles(B, M): the caller's partial buffer fits
-  const int Cp = padded_channels(C);
-  return with_dtype(dtype, [&](auto t) {
-    using T = typename decltype(t)::type;
-    const T* gy = static_cast<const T*>(grad_y);
-    bn_relu_bwd_stats_kernel<T><<<ntiles, 256, 0, stream>>>(gy, x, save_stats, gamma, beta, C, M, partial); CL3D_LAUNCHED(1);
-    const int rc = cl3d_reduce_partials(partial, ntiles, 2 * C, dgamma_dbeta, stream_);  // (dgamma, dbeta)
-    if (rc) return rc;
-    bn_relu_bwd_apply_kernel<T><<<ntiles, 256, 0, stream>>>(gy, x, save_stats, gamma, beta, dgamma_dbeta, C, Cp, M,
-                                                            1.0f / (float)((long long)B * M), training, g_pm); CL3D_LAUNCHED(1);
-    return check_launch("bn_relu_bwd kernels");
-  });
+  const int rc = cl3d_bn_relu_bwd_stats(grad_y, dtype, x, save_stats, gamma, beta, B, C, M, partial, dgamma_dbeta,
+                                        stream_);
+  if (rc) return rc;
+  return cl3d_bn_relu_bwd_apply(grad_y, dtype, x, save_stats, gamma, beta, B, C, M, training, dgamma_dbeta, nullptr,
+                                nullptr, g_pm, stream_);
 }

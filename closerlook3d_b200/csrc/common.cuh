@@ -134,6 +134,9 @@ __device__ __forceinline__ int warp_sum_i(int v) {
 // variance: a raw fp32 sum of squares loses (mean/std)^2 * 2^-24 of it, a raw fp32 tile sum ~ 2^-24 * |mean| of the
 // tile mean, and both cancel in the finalize.  cl3d_bn_finalize merges the tiles in double.
 constexpr int kBnRows = CL3D_BN_PARTIAL_ROWS;
+// out[i] = sums[i] * (1 / *count) for the BatchNorm backward's apply passes when the count is held on the device
+// (cross-rank statistics): they then run with inv_count = 1 (bn.cu)
+int bn_mean_terms(const float* sums, int n, const double* count, float* out, cudaStream_t stream);
 
 __device__ __forceinline__ void store_bn_moments(float* partial, size_t tile, int C, int c, float n, float ctr,
                                                  float d, float q) {

@@ -638,10 +638,11 @@ static PwQueryLaunch pw_query_launch(int B, int M, int Cop) {
           (size_t)ny * 3 * Cop * sizeof(float)};
 }
 
-// Backward scratch, parts 64-float aligned: [ partials | sc*dz (B,M,Cop) | d/da' (B,M,Cop), deterministic mode only ].
-// The partials are the statistics pass's (2 rows of Cout per query tile), then the query pass's d/dWp (3 rows per CTA).
+// Backward scratch, parts 64-float aligned: [ partials | sc*dz (B,M,Cop) | d/da' (B,M,Cop), deterministic mode only |
+// the (2,Cout) means of a device-held count ].  The partials are the statistics pass's (2 rows of Cout per query tile),
+// then the query pass's d/dWp (3 rows per CTA).
 struct PwScratch {
-  size_t dzs, da, floats;  // offsets of sc*dz and d/da' (the partials start at 0); the size
+  size_t dzs, da, means, floats;  // offsets of sc*dz, d/da' and the means (the partials start at 0); the size
 };
 static PwScratch pw_scratch(int B, int M, int Cout, int deterministic) {
   const int Cop = padded_channels(Cout);
@@ -650,7 +651,8 @@ static PwScratch pw_scratch(int B, int M, int Cout, int deterministic) {
   PwScratch s;
   s.dzs = align_up((stats_rows > wp_rows ? stats_rows : wp_rows) * Cout, 64);
   s.da = s.dzs + align_up(pm, 64);
-  s.floats = deterministic ? s.da + pm : s.dzs + pm;
+  s.means = deterministic ? s.da + align_up(pm, 64) : s.da;
+  s.floats = s.means + 2 * (size_t)Cout;
   return s;
 }
 
@@ -750,83 +752,105 @@ static PwEvents* pw_events() {
   return &ring[dev][next[dev]++ % kRing];
 }
 
-extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta, const float* ab_pm,
-                              const float* wp, const float* sgn, const float* query_xyz, const float* support_xyz,
-                              const int* idx, const int* csr_off, const int* csr_ent, const float* ysel,
-                              const float* aq, const float* sq, const unsigned char* karg, const float* save_stats,
-                              const float* gamma, int B, int N, int M, int K, int Cout, float radius, int training,
-                              int deterministic, float* scratch, float* dgamma_dbeta, float* grad_ab_pm,
-                              float* grad_wp, cl3d_stream_t stream_, cl3d_stream_t side_stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
+// The backward's arguments, shared by its two halves (cl3d_pwmlp_bwd_stats | cl3d_pwmlp_bwd_apply) and the unsplit call
+struct PwBwdCall {
+  const void* grad_out;
+  int dtype;
+  const float *beta, *ab_pm, *wp, *sgn, *query_xyz, *support_xyz;
+  const int *idx, *csr_off, *csr_ent;
+  const float *ysel, *aq, *sq;
+  const unsigned char* karg;
+  const float *save_stats, *gamma;
+  int B, N, M, K, Cout;
+  float radius;
+  int training, deterministic;
+  float* scratch;
+  float* dgamma_dbeta;   // the statistics half's output
+  const float* dgb;      // the apply half's (sum dz*yhat, sum dz)
+  const double* count;   // the apply half's count on the device, or NULL: B*M*K
+  float *grad_ab_pm, *grad_wp;
+  cudaStream_t stream, side;
+};
+
+// run_stats: the statistics pass + its reduction into dgamma_dbeta;  run_apply: the dense / query / gather passes.
+// The zero-fill of grad_ab is forked onto the side stream first, so that in the unsplit call it overlaps the
+// statistics pass.
+static int pw_bwd(const PwBwdCall& p, bool run_stats, bool run_apply) {
+  cudaStream_t stream = p.stream;
   // With a side stream the zero-fill of grad_ab and the latency-bound query pass run beside the statistics and
   // the support-major gather (fork/join with events: capturable into a CUDA graph); without one, in order.
   // Deterministic mode runs in order on `stream`: its gather pass reads the query pass's da'.
-  cudaStream_t side = side_stream_ && !deterministic ? (cudaStream_t)side_stream_ : stream;
+  cudaStream_t side = run_apply && p.side && !p.deterministic ? p.side : stream;
   const bool forked = side != stream;
   PwEvents* ev = forked ? pw_events() : nullptr;
   if (forked && !ev) return CL3D_ERR_LAUNCH;
-  CL3D_REQUIRE_DTYPE(dtype, "cl3d_pwmlp_bwd");
-  CL3D_REQUIRE(grad_out && beta && ab_pm && wp && sgn && query_xyz && support_xyz && idx && ysel && aq && sq &&
-                   karg && save_stats && gamma && scratch && dgamma_dbeta && grad_ab_pm && grad_wp,
-               "cl3d_pwmlp_bwd: null pointer");
-  CL3D_REQUIRE((!training && !deterministic) || (csr_off && csr_ent),
-               "cl3d_pwmlp_bwd: training or deterministic mode needs the all-slots CSR lists");
-  CL3D_REQUIRE(B >= 0 && N >= 1 && M >= 1 && K >= 1 && K <= 255 && Cout >= 1, "cl3d_pwmlp_bwd: bad sizes");
+  const int B = p.B, N = p.N, M = p.M, K = p.K, Cout = p.Cout;
   if (B == 0) return CL3D_OK;
   const int ntiles = B * ceil_div(M, kPWTile);
   const int ntn = B * ceil_div(N, kPWTile);
   const int gx = pw_dense_grid(ntn);
   const int Cop = padded_channels(Cout);
   const PwQueryLaunch ql = pw_query_launch(B, M, Cop);
-  const PwScratch sl = pw_scratch(B, M, Cout, deterministic);
-  float* partial = scratch;
-  float* dzs_pm = scratch + sl.dzs;
-  float* da_pm = scratch + sl.da;  // deterministic mode only
+  const PwScratch sl = pw_scratch(B, M, Cout, p.deterministic);
+  float* partial = p.scratch;
+  float* dzs_pm = p.scratch + sl.dzs;
+  float* da_pm = p.scratch + sl.da;  // deterministic mode only
   const size_t smem_s = (size_t)kPWTile * (Cop + 1) * sizeof(float);
   if (forked) {
     cudaEventRecord(ev->start, stream);
     cudaStreamWaitEvent(side, ev->start, 0);
   }
-  if (!deterministic) cudaMemsetAsync(grad_ab_pm, 0, sizeof(float) * (size_t)B * N * 2 * Cop, side);
+  if (run_apply && !p.deterministic) cudaMemsetAsync(p.grad_ab_pm, 0, sizeof(float) * (size_t)B * N * 2 * Cop, side);
   if (forked) cudaEventRecord(ev->zeroed, side);
-  with_dtype(dtype, [&](auto t) {
-    using TG = typename decltype(t)::type;
-    const TG* g = static_cast<const TG*>(grad_out);
-    static std::atomic<unsigned long long> seen_stats{0};
-    allow_big_smem(pwmlp_bwd_stats_kernel<TG>, seen_stats);
-    pwmlp_bwd_stats_kernel<TG><<<ntiles, 256, smem_s, stream>>>(g, ysel, save_stats, gamma, Cout, Cop, M, partial, dzs_pm,
-                                                                beta);
-    return CL3D_OK;
-  });
-  CL3D_LAUNCHED(1);
-  int rc = cl3d_reduce_partials(partial, ntiles, 2 * Cout, dgamma_dbeta, stream_);  // (dgamma, dbeta)
-  if (rc) return rc;
+  int rc;
+  if (run_stats) {
+    with_dtype(p.dtype, [&](auto t) {
+      using TG = typename decltype(t)::type;
+      const TG* g = static_cast<const TG*>(p.grad_out);
+      static std::atomic<unsigned long long> seen_stats{0};
+      allow_big_smem(pwmlp_bwd_stats_kernel<TG>, seen_stats);
+      pwmlp_bwd_stats_kernel<TG><<<ntiles, 256, smem_s, stream>>>(g, p.ysel, p.save_stats, p.gamma, Cout, Cop, M, partial,
+                                                                  dzs_pm, p.beta);
+      return CL3D_OK;
+    });
+    CL3D_LAUNCHED(1);
+    rc = cl3d_reduce_partials(partial, ntiles, 2 * Cout, p.dgamma_dbeta, stream);  // (dgamma, dbeta)
+    if (rc) return rc;
+  }
+  if (!run_apply) return check_launch("pwmlp_bwd_stats_kernel");
+  PwArgs a = {};
+  a.ab_pm = p.ab_pm; a.wp = p.wp; a.sgn = p.sgn; a.query_xyz = p.query_xyz; a.support_xyz = p.support_xyz; a.idx = p.idx;
+  a.ysel = const_cast<float*>(p.ysel); a.aq = const_cast<float*>(p.aq); a.sq = const_cast<float*>(p.sq);
+  a.karg = const_cast<unsigned char*>(p.karg);
+  a.partial = partial;
+  a.stats = p.save_stats; a.gamma = p.gamma; a.dgb = p.dgb;
+  a.csr_off = p.csr_off; a.csr_ent = p.csr_ent;
+  a.grad_ab_pm = p.grad_ab_pm;
+  a.dzs_pm = dzs_pm;
+  a.B = B; a.N = N; a.M = M; a.K = K; a.Cout = Cout; a.Cop = Cop;
+  a.inv_radius = 1.0f / p.radius;
+  // eval mode (frozen BatchNorm): the batch-statistics terms c1, c2 vanish (inv_count = 0 zeroes them in the query
+  // pass) and the dense support-major pass would add exact zeros, so it is not launched
+  a.inv_count = p.training ? 1.0f / (float)((double)B * M * K) : 0.f;
+  if (p.training && p.count) {  // the means over the device-held count; the passes then scale by 1
+    float* means = p.scratch + sl.means;
+    rc = bn_mean_terms(p.dgb, 2 * Cout, p.count, means, stream);
+    if (rc) return rc;
+    a.dgb = means;
+    a.inv_count = 1.0f;
+  }
+  a.ntiles = ntn;  // the support-major passes walk tiles of support points
   if (forked) {
     cudaEventRecord(ev->stats, stream);
     cudaStreamWaitEvent(side, ev->stats, 0);   // the query pass needs (dgamma, dbeta) and sc*dz
     cudaStreamWaitEvent(stream, ev->zeroed, 0);  // the gather pass needs the zero-filled grad_ab
   }
-  PwArgs a = {};
-  a.ab_pm = ab_pm; a.wp = wp; a.sgn = sgn; a.query_xyz = query_xyz; a.support_xyz = support_xyz; a.idx = idx;
-  a.ysel = const_cast<float*>(ysel); a.aq = const_cast<float*>(aq); a.sq = const_cast<float*>(sq);
-  a.karg = const_cast<unsigned char*>(karg);
-  a.partial = partial;
-  a.stats = save_stats; a.gamma = gamma; a.dgb = dgamma_dbeta;
-  a.csr_off = csr_off; a.csr_ent = csr_ent;
-  a.grad_ab_pm = grad_ab_pm;
-  a.dzs_pm = dzs_pm;
-  a.B = B; a.N = N; a.M = M; a.K = K; a.Cout = Cout; a.Cop = Cop;
-  a.inv_radius = 1.0f / radius;
-  // eval mode (frozen BatchNorm): the batch-statistics terms c1, c2 vanish (inv_count = 0 zeroes them in the query
-  // pass) and the dense support-major pass would add exact zeros, so it is not launched
-  a.inv_count = training ? 1.0f / (float)((double)B * M * K) : 0.f;
-  a.ntiles = ntn;  // the support-major passes walk tiles of support points
-  if (deterministic) {
+  if (p.deterministic) {
     pwmlp_bwd_query_det_kernel<<<ql.grid, ql.block, ql.smem, stream>>>(a, (long long)B * M, da_pm);
     CL3D_LAUNCHED(1);
     rc = check_launch("pwmlp_bwd_query_det_kernel");
     if (rc) return rc;
-    rc = cl3d_reduce_partials(partial, (int)ql.grid.x, 3 * Cout, grad_wp, stream_);
+    rc = cl3d_reduce_partials(partial, (int)ql.grid.x, 3 * Cout, p.grad_wp, stream);
     if (rc) return rc;
     return with_pw_ci(Cop, [&](auto ci) {
       constexpr int CI = decltype(ci)::value;
@@ -835,7 +859,7 @@ extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta
       return check_launch("pwmlp_bwd_gather_det_kernel");
     });
   }
-  if (training) {
+  if (p.training) {
     rc = with_pw_ci(Cop, [&](auto ci) {
       constexpr int CI = decltype(ci)::value;
       pwmlp_bwd_dense_kernel<CI><<<dim3(gx, ceil_div(Cop, 32 * CI)), kPWWarps * 32, 0, stream>>>(a);
@@ -848,10 +872,64 @@ extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta
   CL3D_LAUNCHED(1);
   rc = check_launch("pwmlp_bwd_query_kernel");
   if (rc) return rc;
-  rc = cl3d_reduce_partials(partial, (int)ql.grid.x, 3 * Cout, grad_wp, (cl3d_stream_t)side);
+  rc = cl3d_reduce_partials(partial, (int)ql.grid.x, 3 * Cout, p.grad_wp, (cl3d_stream_t)side);
   if (forked) {
     cudaEventRecord(ev->joined, side);
     cudaStreamWaitEvent(stream, ev->joined, 0);
   }
   return rc;
+}
+
+extern "C" int cl3d_pwmlp_bwd_stats(const void* grad_out, int dtype, const float* beta, const float* ysel,
+                                    const float* save_stats, const float* gamma, int B, int M, int Cout, float* scratch,
+                                    float* dgamma_dbeta, cl3d_stream_t stream_) {
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_pwmlp_bwd_stats");
+  CL3D_REQUIRE(grad_out && beta && ysel && save_stats && gamma && scratch && dgamma_dbeta,
+               "cl3d_pwmlp_bwd_stats: null pointer");
+  CL3D_REQUIRE(B >= 0 && M >= 1 && Cout >= 1, "cl3d_pwmlp_bwd_stats: bad sizes");
+  PwBwdCall p = {};
+  p.grad_out = grad_out; p.dtype = dtype; p.beta = beta; p.ysel = ysel; p.save_stats = save_stats; p.gamma = gamma;
+  p.B = B; p.N = 1; p.M = M; p.K = 1; p.Cout = Cout;
+  p.scratch = scratch; p.dgamma_dbeta = dgamma_dbeta;
+  p.stream = p.side = (cudaStream_t)stream_;
+  return pw_bwd(p, true, false);
+}
+
+#define PW_BWD_REQUIRE(what, dgb)                                                                                   \
+  CL3D_REQUIRE_DTYPE(dtype, what);                                                                                  \
+  CL3D_REQUIRE(grad_out && beta && ab_pm && wp && sgn && query_xyz && support_xyz && idx && ysel && aq && sq &&     \
+                   karg && save_stats && gamma && scratch && dgb && grad_ab_pm && grad_wp,                          \
+               what ": null pointer");                                                                              \
+  CL3D_REQUIRE((!training && !deterministic) || (csr_off && csr_ent),                                               \
+               what ": training or deterministic mode needs the all-slots CSR lists");                             \
+  CL3D_REQUIRE(B >= 0 && N >= 1 && M >= 1 && K >= 1 && K <= 255 && Cout >= 1, what ": bad sizes")
+
+#define PW_BWD_CALL(dgb_out, dgb_in, count_in)                                                                   \
+  PwBwdCall p = {grad_out, dtype, beta, ab_pm, wp, sgn, query_xyz, support_xyz, idx, csr_off, csr_ent, ysel, aq, \
+                 sq, karg, save_stats, gamma, B, N, M, K, Cout, radius, training, deterministic, scratch,        \
+                 dgb_out, dgb_in, count_in, grad_ab_pm, grad_wp, (cudaStream_t)stream_, (cudaStream_t)side_stream_}
+
+extern "C" int cl3d_pwmlp_bwd_apply(const void* grad_out, int dtype, const float* beta, const float* ab_pm,
+                                    const float* wp, const float* sgn, const float* query_xyz, const float* support_xyz,
+                                    const int* idx, const int* csr_off, const int* csr_ent, const float* ysel,
+                                    const float* aq, const float* sq, const unsigned char* karg,
+                                    const float* save_stats, const float* gamma, int B, int N, int M, int K, int Cout,
+                                    float radius, int training, int deterministic, float* scratch,
+                                    const float* dgb_sums, const double* count, float* grad_ab_pm, float* grad_wp,
+                                    cl3d_stream_t stream_, cl3d_stream_t side_stream_) {
+  PW_BWD_REQUIRE("cl3d_pwmlp_bwd_apply", dgb_sums);
+  PW_BWD_CALL(nullptr, dgb_sums, count);
+  return pw_bwd(p, false, true);
+}
+
+extern "C" int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta, const float* ab_pm,
+                              const float* wp, const float* sgn, const float* query_xyz, const float* support_xyz,
+                              const int* idx, const int* csr_off, const int* csr_ent, const float* ysel,
+                              const float* aq, const float* sq, const unsigned char* karg, const float* save_stats,
+                              const float* gamma, int B, int N, int M, int K, int Cout, float radius, int training,
+                              int deterministic, float* scratch, float* dgamma_dbeta, float* grad_ab_pm,
+                              float* grad_wp, cl3d_stream_t stream_, cl3d_stream_t side_stream_) {
+  PW_BWD_REQUIRE("cl3d_pwmlp_bwd", dgamma_dbeta);
+  PW_BWD_CALL(dgamma_dbeta, dgamma_dbeta, nullptr);
+  return pw_bwd(p, true, true);
 }

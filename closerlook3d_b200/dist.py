@@ -1,8 +1,13 @@
 """Data parallelism of the hot path: clouds are independent, so a batch shards over ranks by the batch
-dimension and the ONLY exchange is the all-reduce of parameter gradients (reference: DistributedSampler +
+dimension and the only exchange is the all-reduce of parameter gradients (reference: DistributedSampler +
 DistributedDataParallel(broadcast_buffers=False), /root/reference/pytorch/function/train_modelnet_dist.py:117,206;
-BatchNorm statistics are per GPU, not synchronised).  One process per GPU, NCCL over NVLink/NVSwitch
-(gloo on CPU in the tests)."""
+BatchNorm statistics are per GPU by default, not synchronised).  One process per GPU, NCCL over NVLink/NVSwitch
+(gloo on CPU in the tests).
+
+A model converted with nn.SyncBatchNorm.convert_sync_batchnorm synchronises its BatchNorm statistics, fused operators
+included: each fused BatchNorm then adds one all_gather of a small float64 record in the forward and one of its
+(sum gy*xhat, sum gy) in the backward, over bn.process_group (ops.bn_sync_group, ops.bn_batch_stats).  dgamma and
+dbeta stay per rank and travel with the parameter-gradient all-reduce.  Shards may be uneven (shard_range)."""
 import torch
 import torch.distributed as dist
 

@@ -48,11 +48,11 @@ class _FusedAggBNReLU(Function):
         agg, partial = ops.agg_fwd(spec.family, spec.reduction, feat_pm, query_xyz, support_xyz, nl.idx, nl.ncount,
                                    p0, p1, C, spec.radius, spec.normalize, spec.shared, spec.nkp, spec.extent,
                                    spec.influence, want_bn_partial=bn.training or bn.running_mean is None, arg=arg)
-        stats, training = ops.bn_batch_stats(bn, partial, C, B * M)
+        stats, training, sync = ops.bn_batch_stats(bn, partial, C, B * M)
         out = ops.bn_relu_fwd(agg, stats, bn_weight, bn_bias, dtype=features.dtype)
         if any(ctx.needs_input_grad):
             nl.prefetch_csr(all_slots=False)      # transposed lists for the backward, built behind the forward
-        ctx.spec, ctx.nl, ctx.training, ctx.N, ctx.dtype = spec, nl, training, N, features.dtype
+        ctx.spec, ctx.nl, ctx.training, ctx.sync, ctx.N, ctx.dtype = spec, nl, training, sync, N, features.dtype
         needs_feat = spec.family in (ops.FAM_ADAPTIVE_DP, ops.FAM_PSEUDOGRID)
         ctx.save_for_backward(agg, stats, bn_weight, bn_bias, query_xyz, support_xyz, p0, p1,
                               feat_pm if needs_feat else None, arg)
@@ -64,7 +64,8 @@ class _FusedAggBNReLU(Function):
         agg, stats, bn_weight, bn_bias, query_xyz, support_xyz, p0, p1, feat_pm, arg = ctx.saved_tensors
         spec, nl = ctx.spec, ctx.nl
         C = agg.shape[1]
-        g_pm, dgamma, dbeta = ops.bn_relu_bwd(grad_out.contiguous(), agg, stats, bn_weight, bn_bias, ctx.training)
+        g_pm, dgamma, dbeta = ops.bn_relu_bwd(grad_out.contiguous(), agg, stats, bn_weight, bn_bias, ctx.training,
+                                              sync=ctx.sync)
         off, ent = nl.csr()
         grad_feat, pg = ops.agg_bwd(spec.family, spec.reduction, g_pm, feat_pm, query_xyz, support_xyz, nl.ncount,
                                     off, ent, p0, p1, C, ctx.N, spec.nsample, spec.radius, spec.normalize,

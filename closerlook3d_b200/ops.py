@@ -293,17 +293,70 @@ def bn_finalize(bn_partial, C, count, eps, momentum, training, running_mean, run
     return stats
 
 
+def bn_sync_group(bn):
+    """The process group over which `bn` synchronises its batch statistics, or None.  torch's SyncBatchNorm rule: `bn`
+    is an nn.SyncBatchNorm in training mode, torch.distributed is initialised, and its process group (bn.process_group,
+    else WORLD) has more than one rank.  The one place that knows about nn.SyncBatchNorm: every other BatchNorm, and a
+    SyncBatchNorm that torch would not synchronise, takes the per-GPU path."""
+    if not (isinstance(bn, torch.nn.SyncBatchNorm) and bn.training):
+        return None
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group or dist.group.WORLD
+    return group if dist.get_world_size(group) > 1 else None
+
+
+def _gather_ranks(t, group):
+    """(R, C) on every rank -> (W, R, C): one all_gather over `group`, rows in rank order"""
+    import torch.distributed as dist
+    W = dist.get_world_size(group)
+    out = torch.empty(W, *t.shape, dtype=t.dtype, device=t.device)
+    dist.all_gather_into_tensor(out.view(W * t.shape[0], *t.shape[1:]), t, group=group)
+    return out
+
+
 def bn_batch_stats(bn, partial, C, count):
     """The BatchNorm statistics a fused forward normalises with, as nn.BatchNorm in `bn`'s mode: batch statistics
     (updating the running ones, momentum=None as a cumulative average) when training or when there are no running
-    statistics, else the running ones.  -> (save_stats (2,C): mean, invstd; training)"""
+    statistics, else the running ones.  -> (save_stats (2,C): mean, invstd; training; sync).
+    sync is None, or (process group, global count (1,) float64 on the device) when `bn` synchronises (bn_sync_group):
+    the statistics are then those of every rank's values, gathered once and merged in rank order on the device."""
     training = bn.training or bn.running_mean is None
     momentum = bn.momentum if bn.momentum is not None else 0.0
     if training and bn.running_mean is not None:
         bn.num_batches_tracked.add_(1)
         if bn.momentum is None:
             momentum = 1.0 / float(bn.num_batches_tracked)
-    return bn_finalize(partial, C, count, bn.eps, momentum, training, bn.running_mean, bn.running_var), training
+    group = bn_sync_group(bn)
+    if group is None:
+        return bn_finalize(partial, C, count, bn.eps, momentum, training, bn.running_mean, bn.running_var), training, None
+    stats, count_all = bn_finalize_ranks(partial, C, count, bn.eps, momentum, bn.running_mean, bn.running_var, group)
+    return stats, training, (group, count_all)
+
+
+@_on_device
+def bn_finalize_ranks(bn_partial, C, count, eps, momentum, running_mean, running_var, group):
+    """Training statistics over every rank of `group`: this rank's (4,C) float64 record of its per-tile moments, one
+    all_gather, the merge in rank order.  -> (save_stats (2,C), global count (1,) float64); updates the running
+    statistics with the global count."""
+    L = _lib.lib()
+    dev = bn_partial.device
+    record = torch.empty(4, C, dtype=torch.float64, device=dev)
+    check(L.cl3d_bn_rank_moments(ptr(bn_partial), bn_partial.shape[0], C, int(count), ptr(record), stream_ptr()),
+          "cl3d_bn_rank_moments")
+    records = _gather_ranks(record, group)
+    stats = torch.empty(2, C, dtype=F32, device=dev)
+    count_all = torch.empty(1, dtype=torch.float64, device=dev)
+    check(L.cl3d_bn_finalize_ranks(ptr(records), records.shape[0], C, float(eps), float(momentum), ptr(running_mean),
+                                   ptr(running_var), ptr(stats), ptr(count_all), stream_ptr()), "cl3d_bn_finalize_ranks")
+    return stats, count_all
+
+
+def _global_sums(dgb, group):
+    """this rank's (2,C) backward sums -> the sums over every rank of `group`, added in rank order"""
+    rows = _gather_ranks(dgb, group)
+    return reduce_partials(rows.view(rows.shape[0], -1))
 
 
 @_on_device
@@ -317,8 +370,10 @@ def bn_relu_fwd(x, stats, gamma, beta, dtype=F32):
 
 
 @_on_device
-def bn_relu_bwd(grad_y, x, stats, gamma, beta, training):
-    """grad_y in the features' dtype -> (g_pm (B,M,Cp) point-major d/d(agg), dgamma (C,), dbeta (C,)), all fp32"""
+def bn_relu_bwd(grad_y, x, stats, gamma, beta, training, sync=None):
+    """grad_y in the features' dtype -> (g_pm (B,M,Cp) point-major d/d(agg), dgamma (C,), dbeta (C,)), all fp32.
+    sync: the forward's (process group, global count): d/d(agg) takes the batch-statistic sums of every rank;
+    dgamma and dbeta stay this rank's"""
     dt = require_features(grad_y, "grad_y")
     B, C, M = x.shape
     L = _lib.lib()
@@ -326,8 +381,16 @@ def bn_relu_bwd(grad_y, x, stats, gamma, beta, training):
     partial = torch.empty(L.cl3d_agg_num_tiles(B, M), 2, C, dtype=F32, device=dev)
     dgb = torch.empty(2, C, dtype=F32, device=dev)
     g_pm = _empty_pm(B, M, padded_channels(C), dev)
-    check(L.cl3d_bn_relu_bwd(ptr(grad_y), dt, ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, int(training),
-                             ptr(partial), ptr(dgb), ptr(g_pm), stream_ptr()), "cl3d_bn_relu_bwd")
+    if sync is None:
+        check(L.cl3d_bn_relu_bwd(ptr(grad_y), dt, ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, int(training),
+                                 ptr(partial), ptr(dgb), ptr(g_pm), stream_ptr()), "cl3d_bn_relu_bwd")
+        return g_pm, dgb[0], dgb[1]
+    group, count = sync
+    check(L.cl3d_bn_relu_bwd_stats(ptr(grad_y), dt, ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, ptr(partial),
+                                   ptr(dgb), stream_ptr()), "cl3d_bn_relu_bwd_stats")
+    sums = _global_sums(dgb, group)
+    check(L.cl3d_bn_relu_bwd_apply(ptr(grad_y), dt, ptr(x), ptr(stats), ptr(gamma), ptr(beta), B, C, M, int(training),
+                                   ptr(sums), ptr(count), ptr(partial), ptr(g_pm), stream_ptr()), "cl3d_bn_relu_bwd_apply")
     return g_pm, dgb[0], dgb[1]
 
 
@@ -405,12 +468,13 @@ def pwmlp_fwd_stats(ab_pm, wp, sgn, query_xyz, support_xyz, idx, Cout, radius):
 
 @_on_device
 def pwmlp_bwd(grad_out, beta, ab_pm, wp, sgn, query_xyz, support_xyz, idx, csr_off, csr_ent, ysel, aq, sq, karg, stats,
-              gamma, radius, side_stream=None, training=True, deterministic=None):
+              gamma, radius, side_stream=None, training=True, deterministic=None, sync=None):
     """grad_out in the features' dtype -> (grad_ab_pm (B,N,2Cop), grad_wp (3,Cout), dgamma (Cout), dbeta (Cout)), fp32;
     the ReLU decision is recomputed from ysel, stats, gamma and beta.  side_stream: a torch stream the library may fork
     onto (zero-fill + query pass run beside the gather pass), joined before it returns.  deterministic (None: torch's
     flag): no atomics, every grad_ab row gathered from the canonical all-slots lists csr_off / csr_ent (required then,
-    in eval mode too)"""
+    in eval mode too).  sync: the forward's (process group, global count): the passes after the statistics take the
+    batch-statistic sums of every rank; dgamma and dbeta stay this rank's"""
     dt = require_features(grad_out, "grad_out")
     B, N, C2 = ab_pm.shape
     Cout, M, K = ysel.shape[1], ysel.shape[2], idx.shape[2]
@@ -421,12 +485,19 @@ def pwmlp_bwd(grad_out, beta, ab_pm, wp, sgn, query_xyz, support_xyz, idx, csr_o
     dgb = torch.empty(2, Cout, dtype=F32, device=dev)
     grad_ab = torch.empty(B, N, C2, dtype=F32, device=dev)
     grad_wp = torch.empty(3, Cout, dtype=F32, device=dev)
-    check(L.cl3d_pwmlp_bwd(ptr(grad_out), dt, ptr(beta), ptr(ab_pm), ptr(wp), ptr(sgn), ptr(query_xyz), ptr(support_xyz), ptr(idx),
-                           ptr(csr_off), ptr(csr_ent), ptr(ysel), ptr(aq), ptr(sq), ptr(karg), ptr(stats), ptr(gamma),
-                           B, N, M, K, Cout, float(radius), int(bool(training)), det, ptr(partial), ptr(dgb), ptr(grad_ab),
-                           ptr(grad_wp),
-                           stream_ptr(), ctypes.c_void_p(side_stream.cuda_stream) if side_stream is not None else None),
-          "cl3d_pwmlp_bwd")
+    side = ctypes.c_void_p(side_stream.cuda_stream) if side_stream is not None else None
+    args = (ptr(grad_out), dt, ptr(beta), ptr(ab_pm), ptr(wp), ptr(sgn), ptr(query_xyz), ptr(support_xyz), ptr(idx),
+            ptr(csr_off), ptr(csr_ent), ptr(ysel), ptr(aq), ptr(sq), ptr(karg), ptr(stats), ptr(gamma),
+            B, N, M, K, Cout, float(radius), int(bool(training)), det, ptr(partial))
+    if sync is None:
+        check(L.cl3d_pwmlp_bwd(*args, ptr(dgb), ptr(grad_ab), ptr(grad_wp), stream_ptr(), side), "cl3d_pwmlp_bwd")
+        return grad_ab, grad_wp, dgb[0], dgb[1]
+    group, count = sync
+    check(L.cl3d_pwmlp_bwd_stats(ptr(grad_out), dt, ptr(beta), ptr(ysel), ptr(stats), ptr(gamma), B, M, Cout,
+                                 ptr(partial), ptr(dgb), stream_ptr()), "cl3d_pwmlp_bwd_stats")
+    sums = _global_sums(dgb, group)
+    check(L.cl3d_pwmlp_bwd_apply(*args, ptr(sums), ptr(count), ptr(grad_ab), ptr(grad_wp), stream_ptr(), side),
+          "cl3d_pwmlp_bwd_apply")
     return grad_ab, grad_wp, dgb[0], dgb[1]
 
 

@@ -9,7 +9,8 @@ and num_batches_tracked.
 
 The fused path is taken when the input allows it: x is a CUDA fp32 (B,C,N) tensor, padded C <= 128, every
 num_parts <= 64, at most 32 heads, and all head BatchNorms share one mode, momentum and eps and track running
-statistics.  Any other input runs the reference's own composition of torch modules.
+statistics.  Any other input runs the reference's own composition of torch modules, and so does a head whose BatchNorm
+is an nn.SyncBatchNorm that synchronises (ops.bn_sync_group): the fused kernel keeps its statistics per GPU.
 """
 import torch
 
@@ -37,6 +38,8 @@ def fused_eligible(heads, x):
         if conv1.weight.shape[:2] != (C, C) or conv2.weight.shape[1] != C:
             return False
         if not (bn.track_running_stats and bn.running_mean is not None and bn.affine):
+            return False
+        if ops.bn_sync_group(bn) is not None:   # cross-rank statistics: torch's SyncBatchNorm in the composition
             return False
         if (bn.training, bn.momentum, bn.eps) != (bn0.training, bn0.momentum, bn0.eps):
             return False

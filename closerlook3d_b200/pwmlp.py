@@ -31,9 +31,10 @@ class _FusedPointWiseMLP(Function):
         if any(ctx.needs_input_grad) and (bn.training or bn.running_mean is None or ops.deterministic_mode()):
             nl.prefetch_csr(all_slots=True)         # lists for the backward, built behind the forward kernels
         ysel, aq, sq, karg, partial = ops.pwmlp_fwd_stats(ab_pm, wp, sgn, query_xyz, support_xyz, nl.idx, Cout, radius)
-        stats, training = ops.bn_batch_stats(bn, partial, Cout, B * M * K)
+        stats, training, sync = ops.bn_batch_stats(bn, partial, Cout, B * M * K)
         out = ops.bn_relu_fwd(ysel, stats, bn_weight, bn_bias, dtype=features.dtype)
-        ctx.nl, ctx.radius, ctx.training, ctx.dims = nl, radius, training, (B, C, N, M, K, Cout, Cop, Cpa)
+        ctx.nl, ctx.radius, ctx.training, ctx.sync = nl, radius, training, sync
+        ctx.dims = (B, C, N, M, K, Cout, Cop, Cpa)
         ctx.dtype = features.dtype
         # the backward recomputes the ReLU decision from ysel and the BatchNorm constants, not from `out`
         ctx.save_for_backward(fa_pm, ab_pm, wp, sgn, wcat, ysel, aq, sq, karg, stats, bn_weight, bn_bias, query_xyz,
@@ -54,7 +55,8 @@ class _FusedPointWiseMLP(Function):
         side = pt_utils._side_stream(ysel.device, priority=-1) if pt_utils.overlap_enabled else None
         grad_ab, grad_wp, dgamma, dbeta = ops.pwmlp_bwd(grad_out.contiguous(), bn_bias, ab_pm, wp, sgn, query_xyz, support_xyz, nl.idx,
                                                         off, ent, ysel, aq, sq, karg, stats, bn_weight, ctx.radius,
-                                                        side_stream=side, training=ctx.training, deterministic=det)
+                                                        side_stream=side, training=ctx.training, deterministic=det,
+                                                        sync=ctx.sync)
         P = B * N
         Cp = ops.padded_channels(C)
         # the two products of the backward are independent: the weight gradient runs on the side stream

@@ -238,6 +238,27 @@ int cl3d_bn_relu_fwd(const float* x, const float* save_stats, const float* gamma
 int cl3d_bn_relu_bwd(const void* grad_y, int dtype, const float* x, const float* save_stats, const float* gamma,
                      const float* beta, int B, int C, int M, int training, float* partial /*(ntiles,2,C)*/,
                      float* dgamma_dbeta /*(2,C)*/, float* g_pm /*(B,M,Cp)*/, cl3d_stream_t stream);
+/* cl3d_bn_relu_bwd is its two halves in sequence:
+ *   bwd_stats: the statistics pass and its reduction -> dgamma_dbeta (2,C) = this call's (sum gy*xhat, sum gy).
+ *   bwd_apply: the apply pass with dgb_sums (2,C) = (sum gy*xhat, sum gy) over the whole batch and their count:
+ *              count = NULL -> B*M; else a device float64 (cl3d_bn_finalize_ranks' count), and work (2,C) floats
+ *              receives the means.  Between the halves a caller may exchange and add the sums of several ranks.
+ * Cross-rank statistics (SyncBatchNorm).  Each rank of W turns its forward partials into a (4,C) float64 record
+ * (count, centre, sum (x - centre), sum (x - centre)^2: counts beyond 2^24 stay exact), the W records are gathered in
+ * rank order, and every rank merges them in that order about rank 0's centre: the same merge as cl3d_bn_finalize,
+ * so all ranks get the same bits.  bn_finalize_ranks (training only) writes save_stats, updates the running statistics
+ * with the global count (running_* may be NULL) and stores that count in *count (one float64). */
+int cl3d_bn_relu_bwd_stats(const void* grad_y, int dtype, const float* x, const float* save_stats, const float* gamma,
+                           const float* beta, int B, int C, int M, float* partial /*(ntiles,2,C)*/,
+                           float* dgamma_dbeta /*(2,C)*/, cl3d_stream_t stream);
+int cl3d_bn_relu_bwd_apply(const void* grad_y, int dtype, const float* x, const float* save_stats, const float* gamma,
+                           const float* beta, int B, int C, int M, int training, const float* dgb_sums /*(2,C)*/,
+                           const double* count, float* work /*(2,C)*/, float* g_pm /*(B,M,Cp)*/, cl3d_stream_t stream);
+int cl3d_bn_rank_moments(const float* bn_partial /*(ntiles,CL3D_BN_PARTIAL_ROWS,C)*/, int ntiles, int C, long long count,
+                         double* record /*(4,C)*/, cl3d_stream_t stream);
+int cl3d_bn_finalize_ranks(const double* records /*(W,4,C)*/, int W, int C, float eps, float momentum,
+                           float* running_mean, float* running_var, float* save_stats /*(2,C)*/, double* count,
+                           cl3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused PointWiseMLP (feature_type='dp_fi_df', num_mlps=1, reduction='max';
@@ -306,6 +327,22 @@ int cl3d_pwmlp_bwd(const void* grad_out, int dtype, const float* beta, const flo
                    int M, int K, int Cout, float radius, int training, int deterministic, float* scratch,
                    float* dgamma_dbeta, float* grad_ab_pm, float* grad_wp, cl3d_stream_t stream,
                    cl3d_stream_t side_stream);
+/* cl3d_pwmlp_bwd is its two halves in sequence (the unsplit call also overlaps the zero-fill with the first):
+ *   bwd_stats: the statistics pass (sc*dz into the scratch) and its reduction -> dgamma_dbeta (2,Cout) = this call's
+ *              (sum dz*yhat, sum dz).  Only grad_out, beta, ysel, save_stats and gamma are read.
+ *   bwd_apply: the dense, query and (deterministic) gather passes with dgb_sums (2,Cout) over the whole batch and
+ *              their count: NULL -> B*M*K, else a device float64 (cl3d_bn_finalize_ranks' count).  The same scratch,
+ *              after bwd_stats on it. */
+int cl3d_pwmlp_bwd_stats(const void* grad_out, int dtype, const float* beta, const float* ysel, const float* save_stats,
+                         const float* gamma, int B, int M, int Cout, float* scratch, float* dgamma_dbeta,
+                         cl3d_stream_t stream);
+int cl3d_pwmlp_bwd_apply(const void* grad_out, int dtype, const float* beta, const float* ab_pm, const float* wp,
+                         const float* sgn, const float* query_xyz, const float* support_xyz, const int* idx,
+                         const int* csr_off, const int* csr_ent, const float* ysel, const float* aq, const float* sq,
+                         const unsigned char* karg, const float* save_stats, const float* gamma, int B, int N,
+                         int M, int K, int Cout, float radius, int training, int deterministic, float* scratch,
+                         const float* dgb_sums, const double* count, float* grad_ab_pm, float* grad_wp,
+                         cl3d_stream_t stream, cl3d_stream_t side_stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused multi-shape part-segmentation head (multihead.cu).  Replaces the S per-shape heads of
