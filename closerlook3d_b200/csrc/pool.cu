@@ -6,8 +6,11 @@
 //           coalesced loads; max over ALL K slots (the reference ignores masks here; cyclic padding duplicates
 //           cannot change a max), first arg-max slot kept (max_pool2d's tie rule) for the backward.
 // backward: grad_f[b, c, idx[b,q,arg]] += grad_out[b,c,q]  -- one fp32 red.add row per query into a zeroed
-//           point-major buffer (the reference scatters K times as many atomics through group_points_grad); or, given
-//           the transposed lists of idx, the same sum gathered per support point in list order (deterministic mode).
+//           point-major buffer (the reference scatters K times as many atomics through group_points_grad); a CTA stages
+//           the grad_out of its 32 queries in shared memory, 32 x (C + 1) floats, so a layer wider than the 227 KB
+//           opt-in allows (C > 1815: the width x2 network's layer4 pool, C = 2304) runs as equal channel chunks of a
+//           multiple of 32 over blockIdx.y; or, given the transposed lists of idx, the same sum gathered per support
+//           point in list order (deterministic mode).
 #include "common.cuh"
 
 namespace cl3d {
@@ -86,29 +89,31 @@ __global__ void __launch_bounds__(kPoolWarps * 32) gather_max_fwd_kernel(const f
   }
 }
 
-// grad_pm[b, idx[b,q,arg[b,q,c]], c] += grad_out[b,c,q]
+// grad_pm[b, idx[b,q,arg[b,q,c]], c] += grad_out[b,c,q] for the channels c0 <= c < c0 + chunk of blockIdx.y
 template <typename T>
 __global__ void __launch_bounds__(256) gather_max_bwd_kernel(const T* __restrict__ grad_out,
                                                              const int* __restrict__ idx,
                                                              const unsigned char* __restrict__ arg, int N, int M, int K,
-                                                             int C, int Cp, float* __restrict__ grad_pm) {
-  extern __shared__ float s_g[];  // [32 queries][C + 1]
+                                                             int C, int Cp, int chunk, float* __restrict__ grad_pm) {
+  extern __shared__ float s_g[];  // [32 queries][Cc + 1]
   const int tiles_per_cloud = (M + 31) / 32;
   const int b = blockIdx.x / tiles_per_cloud;
   const int q0 = (blockIdx.x % tiles_per_cloud) * 32;
+  const int c0 = blockIdx.y * chunk;
+  const int Cc = min(chunk, C - c0);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int c = warp; c < C; c += 8) {
-    const int q = q0 + lane;
-    s_g[(size_t)lane * (C + 1) + c] = q < M ? load_f32(grad_out + ((size_t)b * C + c) * M + q) : 0.f;
-  }
+  const T* g = grad_out + ((size_t)b * C + c0) * M + q0;
+  for (int c = warp; c < Cc; c += 8)
+    s_g[(size_t)lane * (Cc + 1) + c] = q0 + lane < M ? load_f32(g + (size_t)c * M + lane) : 0.f;
   __syncthreads();
+  const unsigned char* a = arg + ((size_t)b * M + q0) * Cp + c0;
+  const int* id = idx + ((size_t)b * M + q0) * K;
+  float* gp = grad_pm + (size_t)b * N * Cp + c0;
   for (int ql = warp; ql < 32; ql += 8) {
-    const int q = q0 + ql;
-    if (q >= M) continue;
-    const size_t gq = (size_t)b * M + q;
-    for (int c = lane; c < C; c += 32) {
-      const int j = idx[gq * K + arg[gq * Cp + c]];
-      atomicAdd(grad_pm + ((size_t)b * N + j) * Cp + c, s_g[(size_t)ql * (C + 1) + c]);
+    if (q0 + ql >= M) continue;
+    for (int c = lane; c < Cc; c += 32) {
+      const int j = id[ql * K + a[(size_t)ql * Cp + c]];
+      atomicAdd(gp + (size_t)j * Cp + c, s_g[(size_t)ql * (Cc + 1) + c]);
     }
   }
 }
@@ -203,13 +208,21 @@ extern "C" int cl3d_gather_max_bwd(const void* grad_out, int dtype, const int* i
     });
   }
   cudaMemsetAsync(grad_pm, 0, sizeof(float) * (size_t)B * N * Cp, stream);
-  const size_t smem = (size_t)32 * (C + 1) * sizeof(float);
+  // all C channels in one CTA while its 32 x (C + 1) staged floats fit (C <= 1815), else the fewest equal chunks of a
+  // multiple of 32 channels that do
+  int chunk = C;
+  if ((size_t)32 * (C + 1) * sizeof(float) > (size_t)kMaxDynSmem) {
+    const int most = (kMaxDynSmem / (32 * (int)sizeof(float)) - 1) / 32 * 32;
+    chunk = ceil_div(ceil_div(C, ceil_div(C, most)), 32) * 32;
+  }
+  const size_t smem = (size_t)32 * (chunk + 1) * sizeof(float);
+  const dim3 grid(B * ceil_div(M, 32), ceil_div(C, chunk));
   return with_dtype(dtype, [&](auto t) {
     using T = typename decltype(t)::type;
     static std::atomic<unsigned long long> seen{0};
     allow_big_smem(gather_max_bwd_kernel<T>, seen);
-    gather_max_bwd_kernel<T><<<B * ceil_div(M, 32), 256, smem, stream>>>(static_cast<const T*>(grad_out), idx, arg, N, M,
-                                                                          K, C, Cp, grad_pm);
+    gather_max_bwd_kernel<T><<<grid, 256, smem, stream>>>(static_cast<const T*>(grad_out), idx, arg, N, M, K, C, Cp,
+                                                          chunk, grad_pm);
     CL3D_LAUNCHED(1);
     return check_launch("gather_max_bwd_kernel");
   });
