@@ -67,8 +67,8 @@ SIGNATURES = {
     "cl3d_mhead_save_floats": (_sz, [_i, _i]),
     "cl3d_mhead_fwd_workspace_bytes": (_sz, [_vp, _i, _i]),
     "cl3d_mhead_bwd_workspace_bytes": (_sz, [_vp, _i, _i]),
-    "cl3d_mhead_fwd": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _f, _f, _i, _vp, _vp, _vp, _sz, _vp]),
-    "cl3d_mhead_bwd": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "cl3d_mhead_fwd": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _f, _f, _i, _vp, _vp, _vp, _sz, _vp]),
+    "cl3d_mhead_bwd": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
 MHEAD_MAX_HEADS = 32       # CL3D_MHEAD_MAX_HEADS

@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(1024) reduce_partials_kernel(const float* __re
 
 using namespace cl3d;
 
-extern "C" int cl3d_version(void) { return 105; }
+extern "C" int cl3d_version(void) { return 106; }
 extern "C" const char* cl3d_last_error(void) { return g_err; }
 extern "C" int cl3d_padded_channels(int C) { return padded_channels(C); }
 extern "C" int cl3d_sm_count(void) { return sm_count(); }

@@ -24,6 +24,10 @@
 //                        bits (no recomputation of y), accumulated over the heads in registers, written once.
 // Arithmetic is fp32 FFMA (register-blocked, 4 points x CE/8 rows per thread); reductions over points are per-CTA
 // partials summed in a fixed order: no float atomics, repeat runs are bit-identical.
+// x, the logits, d/dlogits and d/dx may be fp16 or bf16 (template parameter T of the kernels that touch them): they
+// are widened exactly where they are loaded and rounded once where they are stored; everything else stays fp32.
+#include <string.h>
+
 #include "common.cuh"
 
 namespace cl3d {
@@ -37,7 +41,7 @@ struct MhArgs {
   int S, C, NPT;
   int np[CL3D_MHEAD_MAX_HEADS];
   int off[CL3D_MHEAD_MAX_HEADS + 1];
-  const float* g[CL3D_MHEAD_MAX_HEADS];
+  const void* g[CL3D_MHEAD_MAX_HEADS];  // d/dlogits in the boundary type T of the backward kernels
   float* rm[CL3D_MHEAD_MAX_HEADS];
   float* rv[CL3D_MHEAD_MAX_HEADS];
   long long* nbt[CL3D_MHEAD_MAX_HEADS];
@@ -54,21 +58,55 @@ struct MhCfg {
 // save layout (floats): per head [mean | invstd | sc | sh | c0] (5C) | ref (C) | shift (C) | m1 (C) | M2 (C*C)
 __host__ __device__ inline size_t mh_ref_off(int S, int C) { return (size_t)5 * S * C; }
 
+// ---- boundary loads and stores ----------------------------------------------------------------------
+// read-only element load, widened to fp32 (exact)
+__device__ __forceinline__ float mh_ldg(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float mh_ldg(const __half* p) { return __half2float(__ldg(p)); }
+__device__ __forceinline__ float mh_ldg(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+
+// o[0..3] = v0..v3, rounded once to the element type: one 16-byte store for fp32, one 8-byte store for 16 bits.
+// o must be aligned to 4 elements (mh_vec_store).
+template <typename P2>
+__device__ __forceinline__ uint32_t mh_bits(P2 v) {
+  uint32_t u;
+  memcpy(&u, &v, sizeof(u));
+  return u;
+}
+__device__ __forceinline__ void mh_store4(float* o, float v0, float v1, float v2, float v3) {
+  *reinterpret_cast<float4*>(o) = make_float4(v0, v1, v2, v3);
+}
+__device__ __forceinline__ void mh_store4(__half* o, float v0, float v1, float v2, float v3) {
+  *reinterpret_cast<uint2*>(o) = make_uint2(mh_bits(__floats2half2_rn(v0, v1)), mh_bits(__floats2half2_rn(v2, v3)));
+}
+__device__ __forceinline__ void mh_store4(__nv_bfloat16* o, float v0, float v1, float v2, float v3) {
+  *reinterpret_cast<uint2*>(o) =
+      make_uint2(mh_bits(__floats2bfloat162_rn(v0, v1)), mh_bits(__floats2bfloat162_rn(v2, v3)));
+}
+// Whether the rows of a (rows, N) output starting at `base` take mh_store4 at every point index n = 4i: N % 4 == 0
+// puts every row start and every 4i at a multiple of 4 elements from `base`; a 16-bit base must then be 8-byte aligned
+// (fp32 keeps its former rule, N % 4 alone, which assumes a 16-byte aligned buffer as torch allocates).  A row of odd
+// N is only 2-byte aligned in 16 bits, so this depends on N and the address, never on the point index.
+template <typename T>
+__device__ __forceinline__ bool mh_vec_store(const T* base, int N) {
+  return (N & 3) == 0 && (sizeof(T) == 4 || (reinterpret_cast<uintptr_t>(base) & 7) == 0);
+}
+
 // ---- tile loads ---------------------------------------------------------------------------------
 // Xs[c][p] = x[b][c][n0+p] - ref[c] for c < C and valid points, 0 for points past N
-__device__ __forceinline__ void mh_load_x(float* Xs, const float* __restrict__ x, const float* ref, int C, int N,
-                                          int b, int n0) {
+template <typename T>
+__device__ __forceinline__ void mh_load_x(float* Xs, const T* __restrict__ x, const float* ref, int C, int N, int b,
+                                          int n0) {
   for (int e = threadIdx.x; e < C * kMhT; e += kMhThreads) {
     const int c = e / kMhT, p = e - c * kMhT, n = n0 + p;
-    Xs[c * kMhTS + p] = n < N ? __fsub_rn(__ldg(x + ((size_t)b * C + c) * N + n), ref[c]) : 0.f;
+    Xs[c * kMhTS + p] = n < N ? __fsub_rn(mh_ldg(x + ((size_t)b * C + c) * N + n), ref[c]) : 0.f;
   }
 }
 // Ls[j][p] = g[b][j][n0+p] for j < np, 0 for rows np..rows-1 and points past N
-__device__ __forceinline__ void mh_load_g(float* Ls, const float* __restrict__ g, int np, int rows, int N, int b,
-                                          int n0) {
+template <typename T>
+__device__ __forceinline__ void mh_load_g(float* Ls, const T* __restrict__ g, int np, int rows, int N, int b, int n0) {
   for (int e = threadIdx.x; e < rows * kMhT; e += kMhThreads) {
     const int j = e / kMhT, p = e - j * kMhT, n = n0 + p;
-    Ls[j * kMhTS + p] = (j < np && n < N) ? __ldg(g + ((size_t)b * np + j) * N + n) : 0.f;
+    Ls[j * kMhTS + p] = (j < np && n < N) ? mh_ldg(g + ((size_t)b * np + j) * N + n) : 0.f;
   }
 }
 
@@ -154,15 +192,15 @@ __global__ void __launch_bounds__(256) mh_prep_kernel(MhArgs a, const float* __r
 }
 
 // training: per CTA, m1 = sum (x - s), M2 = sum (x - s)(x - s)^T over its tiles -> partial[blk] = [m1 (C) | M2 (C*C)]
-template <int CE>
-__global__ void __launch_bounds__(kMhThreads) mh_moments_kernel(const float* __restrict__ x, int B, int C, int N,
+template <int CE, typename T>
+__global__ void __launch_bounds__(kMhThreads) mh_moments_kernel(const T* __restrict__ x, int B, int C, int N,
                                                                 float* __restrict__ partial) {
   using Cf = MhCfg<CE>;
   extern __shared__ float4 mh_smem4[];
   float* Xs = reinterpret_cast<float*>(mh_smem4);
   __shared__ float s_shift[CL3D_MHEAD_MAX_CHANNELS];
   for (int e = threadIdx.x; e < Cf::RS * kMhTS; e += kMhThreads) Xs[e] = 0.f;
-  if (threadIdx.x < C) s_shift[threadIdx.x] = x[(size_t)threadIdx.x * N];
+  if (threadIdx.x < C) s_shift[threadIdx.x] = load_f32(x + (size_t)threadIdx.x * N);
   float acc[Cf::MT][Cf::MT] = {};
   float m1 = 0.f;
   const int tpc = ceil_div(N, kMhT), ntiles = B * tpc;
@@ -191,7 +229,8 @@ __global__ void __launch_bounds__(kMhThreads) mh_moments_kernel(const float* __r
 }
 
 // one CTA per head: batch (training) or running (eval) statistics, running-statistics update, folded scale/shift
-__global__ void __launch_bounds__(128) mh_stats_kernel(MhArgs a, const float* __restrict__ x, int N,
+template <typename T>
+__global__ void __launch_bounds__(128) mh_stats_kernel(MhArgs a, const T* __restrict__ x, int N,
                                                        const float* __restrict__ w1, const float* __restrict__ gamma,
                                                        const float* __restrict__ beta, float eps, float momentum,
                                                        int training, long long P, float* __restrict__ save) {
@@ -203,7 +242,7 @@ __global__ void __launch_bounds__(128) mh_stats_kernel(MhArgs a, const float* __
   __shared__ double s_ref[CL3D_MHEAD_MAX_CHANNELS], s_sh[CL3D_MHEAD_MAX_CHANNELS];
   const double dP = (double)P;
   if (c < C) {
-    const float sh = x[(size_t)c * N];
+    const float sh = load_f32(x + (size_t)c * N);
     const float r = training ? (float)((double)sh + (double)m1[c] / dP) : sh;
     s_ref[c] = (double)r;
     s_sh[c] = (double)sh;
@@ -257,13 +296,13 @@ __global__ void __launch_bounds__(128) mh_stats_kernel(MhArgs a, const float* __
 }
 
 // logits of every head for a tile of 128 points
-template <int CE>
-__global__ void __launch_bounds__(kMhThreads) mh_fwd_kernel(MhArgs a, const float* __restrict__ x,
+template <int CE, typename T>
+__global__ void __launch_bounds__(kMhThreads) mh_fwd_kernel(MhArgs a, const T* __restrict__ x,
                                                             const float* __restrict__ W1p,
                                                             const float* __restrict__ W2p,
                                                             const float* __restrict__ b2,
                                                             const float* __restrict__ save, int B, int N,
-                                                            float* __restrict__ logits) {
+                                                            T* __restrict__ logits) {
   using Cf = MhCfg<CE>;
   constexpr int R = Cf::R;
   extern __shared__ float4 mh_smem4[];
@@ -273,7 +312,7 @@ __global__ void __launch_bounds__(kMhThreads) mh_fwd_kernel(MhArgs a, const floa
   const float* ref = save + mh_ref_off(S, C);
   for (int e = threadIdx.x; e < CE * kMhTS; e += kMhThreads) Xs[e] = 0.f;
   const int tpc = ceil_div(N, kMhT), ntiles = B * tpc;
-  const bool vec = (N & 3) == 0;
+  const bool vec = mh_vec_store(logits, N);  // head blocks start at B*N*off[s] elements: a multiple of 4 too
   for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
     const int b = t / tpc, n0 = (t % tpc) * kMhT, n = n0 + 4 * lane;
     __syncthreads();
@@ -298,20 +337,19 @@ __global__ void __launch_bounds__(kMhThreads) mh_fwd_kernel(MhArgs a, const floa
       const int np = a.np[s];
       float lo[8][4] = {};
       mh_gemm_rows<8>(lo, W2p + (size_t)s * kMhMaxParts * CE, CE, warp, 8, np, Zs, CE);
-      float* out = logits + (size_t)B * N * a.off[s];
+      T* out = logits + (size_t)B * N * a.off[s];
 #pragma unroll
       for (int r = 0; r < 8; ++r) {
         const int j = warp + 8 * r;
         if (j < np) {
           const float bj = b2[a.off[s] + j];
-          float* o = out + ((size_t)b * np + j) * N + n;
+          T* o = out + ((size_t)b * np + j) * N + n;
           if (vec) {
-            if (n < N) *reinterpret_cast<float4*>(o) = make_float4(lo[r][0] + bj, lo[r][1] + bj, lo[r][2] + bj,
-                                                                   lo[r][3] + bj);
+            if (n < N) mh_store4(o, lo[r][0] + bj, lo[r][1] + bj, lo[r][2] + bj, lo[r][3] + bj);
           } else {
 #pragma unroll
             for (int q = 0; q < 4; ++q)
-              if (n + q < N) o[q] = lo[r][q] + bj;
+              if (n + q < N) store_f32(o + q, lo[r][q] + bj);
           }
         }
       }
@@ -322,8 +360,8 @@ __global__ void __launch_bounds__(kMhThreads) mh_fwd_kernel(MhArgs a, const floa
 
 // backward phase A, CTA (chunk, head): mask bits and per-CTA partials of G, sum gy, dW2, db2
 // partial row layout: G (S,C,C) | sum gy (S,C) | dW2 (NPT,C) | db2 (NPT)
-template <int CE>
-__global__ void __launch_bounds__(kMhThreads) mh_bwd_a_kernel(MhArgs a, const float* __restrict__ x,
+template <int CE, typename T>
+__global__ void __launch_bounds__(kMhThreads) mh_bwd_a_kernel(MhArgs a, const T* __restrict__ x,
                                                               const float* __restrict__ W1p,
                                                               const float* __restrict__ W2tp,
                                                               const float* __restrict__ save, int B, int N,
@@ -332,7 +370,7 @@ __global__ void __launch_bounds__(kMhThreads) mh_bwd_a_kernel(MhArgs a, const fl
   using Cf = MhCfg<CE>;
   constexpr int R = Cf::R, MT = Cf::MT, RS = Cf::RS, CW = Cf::CW;
   const int s = blockIdx.y;
-  const float* g = a.g[s];
+  const T* g = static_cast<const T*>(a.g[s]);
   if (!g) return;
   extern __shared__ float4 mh_smem4[];
   float* Xs = reinterpret_cast<float*>(mh_smem4);
@@ -533,15 +571,15 @@ __global__ void __launch_bounds__(128) mh_bwd_mx_kernel(MhArgs a, const float* _
 }
 
 // dx for a tile of 128 points, accumulated over the heads in registers
-template <int CE>
-__global__ void __launch_bounds__(kMhThreads) mh_bwd_dx_kernel(MhArgs a, const float* __restrict__ x,
+template <int CE, typename T>
+__global__ void __launch_bounds__(kMhThreads) mh_bwd_dx_kernel(MhArgs a, const T* __restrict__ x,
                                                                const float* __restrict__ W1tp,
                                                                const float* __restrict__ W2tp,
                                                                const float* __restrict__ save,
                                                                const float* __restrict__ Mp,
                                                                const float* __restrict__ v0,
                                                                const uint32_t* __restrict__ mask, int training, int B,
-                                                               int N, float* __restrict__ gx) {
+                                                               int N, T* __restrict__ gx) {
   using Cf = MhCfg<CE>;
   constexpr int R = Cf::R, CW = Cf::CW;
   extern __shared__ float4 mh_smem4[];
@@ -553,7 +591,7 @@ __global__ void __launch_bounds__(kMhThreads) mh_bwd_dx_kernel(MhArgs a, const f
   const long long P = (long long)B * N;
   for (int e = threadIdx.x; e < CE * kMhTS; e += kMhThreads) Us[e] = 0.f;
   const int tpc = ceil_div(N, kMhT), ntiles = B * tpc;
-  const bool vec = (N & 3) == 0;
+  const bool vec = mh_vec_store(gx, N);
   for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
     const int b = t / tpc, n0 = (t % tpc) * kMhT, n = n0 + 4 * lane;
     float acc[R][4] = {};
@@ -570,7 +608,7 @@ __global__ void __launch_bounds__(kMhThreads) mh_bwd_dx_kernel(MhArgs a, const f
       }
     }
     for (int s = 0; s < S; ++s) {
-      const float* g = a.g[s];
+      const T* g = static_cast<const T*>(a.g[s]);
       if (!g) continue;
       const int np = a.np[s], np4 = (np + 3) & ~3;
       const float* hs = save + (size_t)s * 5 * C;
@@ -606,13 +644,13 @@ __global__ void __launch_bounds__(kMhThreads) mh_bwd_dx_kernel(MhArgs a, const f
     for (int r = 0; r < R; ++r) {
       const int c = warp * R + r;
       if (c < C) {
-        float* o = gx + ((size_t)b * C + c) * N + n;
+        T* o = gx + ((size_t)b * C + c) * N + n;
         if (vec) {
-          if (n < N) *reinterpret_cast<float4*>(o) = make_float4(acc[r][0], acc[r][1], acc[r][2], acc[r][3]);
+          if (n < N) mh_store4(o, acc[r][0], acc[r][1], acc[r][2], acc[r][3]);
         } else {
 #pragma unroll
           for (int q = 0; q < 4; ++q)
-            if (n + q < N) o[q] = acc[r][q];
+            if (n + q < N) store_f32(o + q, acc[r][q]);
         }
       }
     }
@@ -701,10 +739,10 @@ static MhPrep mh_prep_layout(float* base, int S, int CE) {
   return p;
 }
 
-template <int CE>
-static int mh_fwd_impl(const MhArgs& a, const float* x, int B, int N, const float* w1, const float* gamma,
+template <int CE, typename T>
+static int mh_fwd_impl(const MhArgs& a, const T* x, int B, int N, const float* w1, const float* gamma,
                        const float* beta, const float* w2, const float* b2, float eps, float momentum, int training,
-                       float* logits, float* save, float* ws, cudaStream_t st) {
+                       T* logits, float* save, float* ws, cudaStream_t st) {
   using Cf = MhCfg<CE>;
   const int S = a.S, C = a.C;
   const long long P = (long long)B * N;
@@ -715,19 +753,19 @@ static int mh_fwd_impl(const MhArgs& a, const float* x, int B, int N, const floa
     const int g = mh_tile_grid(B, N);
     const size_t smem = (size_t)Cf::RS * kMhTS * sizeof(float);
     static std::atomic<unsigned long long> seen{0};
-    allow_big_smem(mh_moments_kernel<CE>, seen);
-    mh_moments_kernel<CE><<<g, kMhThreads, smem, st>>>(x, B, C, N, partial); CL3D_LAUNCHED(1);
+    allow_big_smem(mh_moments_kernel<CE, T>, seen);
+    mh_moments_kernel<CE, T><<<g, kMhThreads, smem, st>>>(x, B, C, N, partial); CL3D_LAUNCHED(1);
     int rc = check_launch("mh_moments_kernel");
     if (rc) return rc;
     rc = cl3d_reduce_partials(partial, g, C + C * C, save + mh_ref_off(S, C) + 2 * C, st);
     if (rc) return rc;
   }
-  mh_stats_kernel<<<S, 128, 0, st>>>(a, x, N, w1, gamma, beta, eps, momentum, training, P, save); CL3D_LAUNCHED(1);
+  mh_stats_kernel<T><<<S, 128, 0, st>>>(a, x, N, w1, gamma, beta, eps, momentum, training, P, save); CL3D_LAUNCHED(1);
   {
     const size_t smem = (size_t)2 * CE * kMhTS * sizeof(float);
     static std::atomic<unsigned long long> seen{0};
-    allow_big_smem(mh_fwd_kernel<CE>, seen);
-    mh_fwd_kernel<CE><<<mh_tile_grid(B, N), kMhThreads, smem, st>>>(a, x, pw.W1p, pw.W2p, b2, save, B, N, logits);
+    allow_big_smem(mh_fwd_kernel<CE, T>, seen);
+    mh_fwd_kernel<CE, T><<<mh_tile_grid(B, N), kMhThreads, smem, st>>>(a, x, pw.W1p, pw.W2p, b2, save, B, N, logits);
     CL3D_LAUNCHED(1);
   }
   return check_launch("mhead forward kernels");
@@ -758,9 +796,9 @@ static MhBwdWs mh_bwd_layout(const MhArgs& a, int CE, int B, int N, float* base)
   return w;
 }
 
-template <int CE>
-static int mh_bwd_impl(const MhArgs& a, const float* x, int B, int N, const float* w1, const float* w2,
-                       const float* save, int training, float* gx, float* gw1, float* ggamma, float* gbeta,
+template <int CE, typename T>
+static int mh_bwd_impl(const MhArgs& a, const T* x, int B, int N, const float* w1, const float* w2,
+                       const float* save, int training, T* gx, float* gw1, float* ggamma, float* gbeta,
                        float* gw2, float* gb2, float* ws, cudaStream_t st) {
   using Cf = MhCfg<CE>;
   const int S = a.S, C = a.C;
@@ -770,8 +808,8 @@ static int mh_bwd_impl(const MhArgs& a, const float* x, int B, int N, const floa
   {
     const size_t smem = (size_t)(2 * Cf::RS + kMhMaxParts) * kMhTS * sizeof(float);
     static std::atomic<unsigned long long> seen{0};
-    allow_big_smem(mh_bwd_a_kernel<CE>, seen);
-    mh_bwd_a_kernel<CE><<<dim3(w.chunks, S), kMhThreads, smem, st>>>(a, x, w.pw.W1p, w.pw.W2tp, save, B, N,
+    allow_big_smem(mh_bwd_a_kernel<CE, T>, seen);
+    mh_bwd_a_kernel<CE, T><<<dim3(w.chunks, S), kMhThreads, smem, st>>>(a, x, w.pw.W1p, w.pw.W2tp, save, B, N,
                                                                       w.partial, w.LA, w.mask);
     CL3D_LAUNCHED(1);
     const int rc = check_launch("mh_bwd_a_kernel");
@@ -792,22 +830,22 @@ static int mh_bwd_impl(const MhArgs& a, const float* x, int B, int N, const floa
   {
     const size_t smem = (size_t)(CE + kMhMaxParts) * kMhTS * sizeof(float) + (size_t)Cf::CW * kMhT * sizeof(uint32_t);
     static std::atomic<unsigned long long> seen{0};
-    allow_big_smem(mh_bwd_dx_kernel<CE>, seen);
-    mh_bwd_dx_kernel<CE><<<mh_tile_grid(B, N), kMhThreads, smem, st>>>(a, x, w.pw.W1tp, w.pw.W2tp, save, w.Mp, w.v0,
+    allow_big_smem(mh_bwd_dx_kernel<CE, T>, seen);
+    mh_bwd_dx_kernel<CE, T><<<mh_tile_grid(B, N), kMhThreads, smem, st>>>(a, x, w.pw.W1tp, w.pw.W2tp, save, w.Mp, w.v0,
                                                                         w.mask, training, B, N, gx);
     CL3D_LAUNCHED(1);
   }
   return check_launch("mhead backward kernels");
 }
 
-#define CL3D_MH_DISPATCH(CE, fn, ...)           \
+#define CL3D_MH_DISPATCH(CE, T, fn, ...)        \
   switch (CE) {                                 \
-    case 16: return fn<16>(__VA_ARGS__);        \
-    case 32: return fn<32>(__VA_ARGS__);        \
-    case 48: return fn<48>(__VA_ARGS__);        \
-    case 72: return fn<72>(__VA_ARGS__);        \
-    case 96: return fn<96>(__VA_ARGS__);        \
-    case 128: return fn<128>(__VA_ARGS__);      \
+    case 16: return fn<16, T>(__VA_ARGS__);     \
+    case 32: return fn<32, T>(__VA_ARGS__);     \
+    case 48: return fn<48, T>(__VA_ARGS__);     \
+    case 72: return fn<72, T>(__VA_ARGS__);     \
+    case 96: return fn<96, T>(__VA_ARGS__);     \
+    case 128: return fn<128, T>(__VA_ARGS__);   \
     default: return CL3D_ERR_UNSUPPORTED;       \
   }
 
@@ -833,14 +871,15 @@ extern "C" size_t cl3d_mhead_bwd_workspace_bytes(const cl3d_mhead_desc* desc_hos
   return mh_bwd_layout(a, CE, B, N, nullptr).total * sizeof(float);
 }
 
-extern "C" int cl3d_mhead_fwd(const cl3d_mhead_desc* desc_host, const float* x, int B, int N, const float* w1,
-                              const float* gamma, const float* beta, const float* w2, const float* b2, float eps,
-                              float momentum, int training, float* logits, float* save, void* workspace,
-                              size_t workspace_bytes, cl3d_stream_t stream_) {
+extern "C" int cl3d_mhead_fwd(const cl3d_mhead_desc* desc_host, const void* x, int dtype, int B, int N,
+                              const float* w1, const float* gamma, const float* beta, const float* w2,
+                              const float* b2, float eps, float momentum, int training, void* logits, float* save,
+                              void* workspace, size_t workspace_bytes, cl3d_stream_t stream_) {
   MhArgs a;
   int CE = 0;
   const int rc = mh_args(desc_host, a, CE, "cl3d_mhead_fwd");
   if (rc != CL3D_OK) return rc;
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_mhead_fwd");
   CL3D_REQUIRE(x && w1 && gamma && beta && w2 && b2 && logits && save && workspace, "cl3d_mhead_fwd: null pointer");
   CL3D_REQUIRE(B >= 1 && N >= 1, "cl3d_mhead_fwd: bad sizes");
   for (int s = 0; s < a.S; ++s) {
@@ -853,17 +892,22 @@ extern "C" int cl3d_mhead_fwd(const cl3d_mhead_desc* desc_host, const float* x, 
   }
   float* ws = static_cast<float*>(workspace);
   cudaStream_t st = (cudaStream_t)stream_;
-  CL3D_MH_DISPATCH(CE, mh_fwd_impl, a, x, B, N, w1, gamma, beta, w2, b2, eps, momentum, training, logits, save, ws, st)
+  return with_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    CL3D_MH_DISPATCH(CE, T, mh_fwd_impl, a, static_cast<const T*>(x), B, N, w1, gamma, beta, w2, b2, eps, momentum,
+                     training, static_cast<T*>(logits), save, ws, st)
+  });
 }
 
-extern "C" int cl3d_mhead_bwd(const cl3d_mhead_desc* desc_host, const float* x, int B, int N, const float* w1,
-                              const float* w2, const float* save, int training, float* grad_x, float* grad_w1,
-                              float* grad_gamma, float* grad_beta, float* grad_w2, float* grad_b2, void* workspace,
-                              size_t workspace_bytes, cl3d_stream_t stream_) {
+extern "C" int cl3d_mhead_bwd(const cl3d_mhead_desc* desc_host, const void* x, int dtype, int B, int N,
+                              const float* w1, const float* w2, const float* save, int training, void* grad_x,
+                              float* grad_w1, float* grad_gamma, float* grad_beta, float* grad_w2, float* grad_b2,
+                              void* workspace, size_t workspace_bytes, cl3d_stream_t stream_) {
   MhArgs a;
   int CE = 0;
   const int rc = mh_args(desc_host, a, CE, "cl3d_mhead_bwd");
   if (rc != CL3D_OK) return rc;
+  CL3D_REQUIRE_DTYPE(dtype, "cl3d_mhead_bwd");
   CL3D_REQUIRE(x && w1 && w2 && save && grad_x && grad_w1 && grad_gamma && grad_beta && grad_w2 && grad_b2 &&
                    workspace,
                "cl3d_mhead_bwd: null pointer");
@@ -874,6 +918,9 @@ extern "C" int cl3d_mhead_bwd(const cl3d_mhead_desc* desc_host, const float* x, 
   }
   float* ws = static_cast<float*>(workspace);
   cudaStream_t st = (cudaStream_t)stream_;
-  CL3D_MH_DISPATCH(CE, mh_bwd_impl, a, x, B, N, w1, w2, save, training, grad_x, grad_w1, grad_gamma, grad_beta, grad_w2,
-                   grad_b2, ws, st)
+  return with_dtype(dtype, [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    CL3D_MH_DISPATCH(CE, T, mh_bwd_impl, a, static_cast<const T*>(x), B, N, w1, w2, save, training,
+                     static_cast<T*>(grad_x), grad_w1, grad_gamma, grad_beta, grad_w2, grad_b2, ws, st)
+  });
 }

@@ -571,23 +571,24 @@ def _mhead_desc(C, num_parts, running_means=None, running_vars=None, nbts=None, 
 
 @_on_device
 def mhead_fwd(x, w1, gamma, beta, w2, b2, num_parts, running_means, running_vars, nbts, eps, momentum, training):
-    """All S heads over x (B,C,N): -> (logits, save).  logits is flat: the concatenation over s of contiguous
-    (B, num_parts[s], N) blocks.  w1 (S,C,C), gamma/beta (S,C), w2 (sum num_parts, C), b2 (sum num_parts).
-    momentum None = cumulative average (needs nbts).  Training updates the running statistics in place and adds one
-    to every num_batches_tracked."""
-    for t, n in ((x, "x"), (w1, "w1"), (gamma, "gamma"), (beta, "beta"), (w2, "w2"), (b2, "b2")):
+    """All S heads over x (B,C,N) f32 / f16 / bf16: -> (logits in x's dtype, save fp32).  logits is flat: the
+    concatenation over s of contiguous (B, num_parts[s], N) blocks.  w1 (S,C,C), gamma/beta (S,C), w2
+    (sum num_parts, C), b2 (sum num_parts), all fp32.  momentum None = cumulative average (needs nbts).  Training
+    updates the running statistics in place and adds one to every num_batches_tracked."""
+    dt = require_features(x, "x")
+    for t, n in ((w1, "w1"), (gamma, "gamma"), (beta, "beta"), (w2, "w2"), (b2, "b2")):
         require_cuda(t, n, F32)
     B, C, N = x.shape
     L = _lib.lib()
     d = _mhead_desc(C, num_parts, running_means, running_vars, nbts)
     dp = ctypes.addressof(d)
-    logits = torch.empty(B * N * sum(num_parts), dtype=F32, device=x.device)
+    logits = torch.empty(B * N * sum(num_parts), dtype=x.dtype, device=x.device)
     save = torch.empty(L.cl3d_mhead_save_floats(len(num_parts), C), dtype=F32, device=x.device)
     wsb = L.cl3d_mhead_fwd_workspace_bytes(dp, B, N)
     if wsb == 0:
         raise RuntimeError("cl3d_mhead_fwd_workspace_bytes: " + L.cl3d_last_error().decode("utf-8", "replace"))
     ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
-    check(L.cl3d_mhead_fwd(dp, ptr(x), B, N, ptr(w1), ptr(gamma), ptr(beta), ptr(w2), ptr(b2), float(eps),
+    check(L.cl3d_mhead_fwd(dp, ptr(x), dt, B, N, ptr(w1), ptr(gamma), ptr(beta), ptr(w2), ptr(b2), float(eps),
                            -1.0 if momentum is None else float(momentum), int(bool(training)), ptr(logits), ptr(save),
                            ptr(ws), wsb, stream_ptr()), "cl3d_mhead_fwd")
     return logits, save
@@ -595,15 +596,21 @@ def mhead_fwd(x, w1, gamma, beta, w2, b2, num_parts, running_means, running_vars
 
 @_on_device
 def mhead_bwd(x, w1, w2, save, num_parts, grads, training):
-    """grads: per head d/dlogits (B, num_parts[s], N) contiguous, or None (zero).
-    -> (grad_x, grad_w1, grad_gamma, grad_beta, grad_w2, grad_b2)"""
+    """grads: per head d/dlogits (B, num_parts[s], N) contiguous in x's dtype, or None (zero).
+    -> (grad_x in x's dtype, grad_w1, grad_gamma, grad_beta, grad_w2, grad_b2 fp32)"""
+    dt = require_features(x, "x")
+    for s, g in enumerate(grads):
+        if g is not None and g.dtype != x.dtype:
+            raise RuntimeError(f"grads[{s}] is {g.dtype}: d/dlogits must have x's dtype ({x.dtype})")
+        if g is not None:
+            require_cuda(g, f"grads[{s}]", x.dtype)
     B, C, N = x.shape
     S = len(num_parts)
     L = _lib.lib()
     d = _mhead_desc(C, num_parts, grads=grads)
     dp = ctypes.addressof(d)
     dev = x.device
-    gx = torch.empty(B, C, N, dtype=F32, device=dev)
+    gx = torch.empty(B, C, N, dtype=x.dtype, device=dev)
     gw1 = torch.empty(S, C, C, dtype=F32, device=dev)
     gg = torch.empty(S, C, dtype=F32, device=dev)
     gb = torch.empty(S, C, dtype=F32, device=dev)
@@ -613,6 +620,6 @@ def mhead_bwd(x, w1, w2, save, num_parts, grads, training):
     if wsb == 0:
         raise RuntimeError("cl3d_mhead_bwd_workspace_bytes: " + L.cl3d_last_error().decode("utf-8", "replace"))
     ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-    check(L.cl3d_mhead_bwd(dp, ptr(x), B, N, ptr(w1), ptr(w2), ptr(save), int(bool(training)), ptr(gx), ptr(gw1),
+    check(L.cl3d_mhead_bwd(dp, ptr(x), dt, B, N, ptr(w1), ptr(w2), ptr(save), int(bool(training)), ptr(gx), ptr(gw1),
                            ptr(gg), ptr(gb), ptr(gw2), ptr(gb2), ptr(ws), wsb, stream_ptr()), "cl3d_mhead_bwd")
     return gx, gw1, gg, gb, gw2, gb2

@@ -7,10 +7,17 @@ one buffer, nothing is copied.  The heads' parameters and buffers stay in the re
 keys unchanged); BatchNorm keeps nn.BatchNorm1d's semantics in both modes, including the running-statistics update
 and num_batches_tracked.
 
-The fused path is taken when the input allows it: x is a CUDA fp32 (B,C,N) tensor, padded C <= 128, every
-num_parts <= 64, at most 32 heads, and all head BatchNorms share one mode, momentum and eps and track running
-statistics.  Any other input runs the reference's own composition of torch modules, and so does a head whose BatchNorm
-is an nn.SyncBatchNorm that synchronises (ops.bn_sync_group): the fused kernel keeps its statistics per GPU.
+The fused path is taken when the input allows it: x is a CUDA fp32, fp16 or bf16 (B,C,N) tensor, padded C <= 128,
+every num_parts <= 64, at most 32 heads, all head parameters and buffers are fp32, and all head BatchNorms share one
+mode, momentum and eps and track running statistics.  Any other input runs the reference's own composition of torch
+modules (so does a head converted wholesale to a 16-bit type), and so does a head whose BatchNorm is an
+nn.SyncBatchNorm that synchronises (ops.bn_sync_group): the fused kernel keeps its statistics per GPU.
+
+16-bit x (what the decoder hands the heads under torch.autocast) follows the library's dtype rule: the logits and
+d/dx come back in x's dtype, d/dlogits must arrive in it, and everything in between -- parameters, BatchNorm
+statistics, saved state, every accumulator -- stays fp32.  So the result is exactly the fp32 head on x.float(), rounded
+once to x's dtype (fp16: inf exactly where that rounding overflows), and the parameter gradients and running
+statistics are the fp32 run's, bit for bit.
 """
 import torch
 
@@ -23,7 +30,7 @@ def _parts(heads):
 
 def fused_eligible(heads, x):
     """whether `multi_shape_heads_forward` takes the fused kernel for this input"""
-    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 3):
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype in ops.DTYPE_CODE and x.dim() == 3):
         return False
     S, C = len(heads), x.shape[1]
     if not (1 <= S <= _lib.MHEAD_MAX_HEADS) or ops.padded_channels(C) > _lib.MHEAD_MAX_CHANNELS:
@@ -51,6 +58,7 @@ def fused_eligible(heads, x):
 
 class _MultiShapeHeads(torch.autograd.Function):
     @staticmethod
+    @ops.no_autocast
     def forward(ctx, x, w1, gamma, beta, w2, b2, meta):
         num_parts, bns, training, momentum, eps = meta
         x = x.contiguous()
@@ -68,6 +76,7 @@ class _MultiShapeHeads(torch.autograd.Function):
         return tuple(outs)
 
     @staticmethod
+    @ops.no_autocast
     def backward(ctx, *grads):
         x, w1, w2, save = ctx.saved_tensors
         grads = [None if g is None else g.contiguous() for g in grads]

@@ -360,6 +360,10 @@ int cl3d_pwmlp_bwd_apply(const void* grad_out, int dtype, const float* beta, con
  *   bwd          : desc_host->grad_logits[s] = d(loss)/d(logits of head s), (B,num_parts[s],N) contiguous, or NULL
  *                  (counts as zero); grad_x (B,C,N) and every parameter gradient are fully written (no float atomics,
  *                  fixed-order reductions: repeat runs are bit-identical).
+ *   dtype        : CL3D_DTYPE_* of x, logits, every grad_logits[s] and grad_x.  Parameters, running statistics, save
+ *                  and the parameter gradients are fp32 whatever it is; a 16-bit run computes exactly the fp32 head on
+ *                  the widened x and d/dlogits and rounds logits and grad_x once.  The workspace sizes do not depend
+ *                  on it.
  * Limits: padded C <= 128, num_parts[s] <= 64, S <= 32; otherwise CL3D_ERR_UNSUPPORTED.
  * ---------------------------------------------------------------------------------------------- */
 #define CL3D_MHEAD_MAX_HEADS 32
@@ -372,17 +376,17 @@ typedef struct cl3d_mhead_desc {
   float* running_mean[CL3D_MHEAD_MAX_HEADS];          /* (C) per head: read in eval, updated in training */
   float* running_var[CL3D_MHEAD_MAX_HEADS];
   long long* num_batches_tracked[CL3D_MHEAD_MAX_HEADS]; /* per head, += 1 in training; may be NULL if momentum >= 0 */
-  const float* grad_logits[CL3D_MHEAD_MAX_HEADS];     /* backward only, see above */
+  const void* grad_logits[CL3D_MHEAD_MAX_HEADS];      /* backward only, in `dtype`, see above */
 } cl3d_mhead_desc;
 size_t cl3d_mhead_save_floats(int S, int C);
 size_t cl3d_mhead_fwd_workspace_bytes(const cl3d_mhead_desc* desc_host, int B, int N);
 size_t cl3d_mhead_bwd_workspace_bytes(const cl3d_mhead_desc* desc_host, int B, int N);
-int cl3d_mhead_fwd(const cl3d_mhead_desc* desc_host, const float* x, int B, int N, const float* w1,
+int cl3d_mhead_fwd(const cl3d_mhead_desc* desc_host, const void* x, int dtype, int B, int N, const float* w1,
                    const float* gamma, const float* beta, const float* w2, const float* b2, float eps,
-                   float momentum, int training, float* logits, float* save, void* workspace,
+                   float momentum, int training, void* logits, float* save, void* workspace,
                    size_t workspace_bytes, cl3d_stream_t stream);
-int cl3d_mhead_bwd(const cl3d_mhead_desc* desc_host, const float* x, int B, int N, const float* w1,
-                   const float* w2, const float* save, int training, float* grad_x, float* grad_w1,
+int cl3d_mhead_bwd(const cl3d_mhead_desc* desc_host, const void* x, int dtype, int B, int N, const float* w1,
+                   const float* w2, const float* save, int training, void* grad_x, float* grad_w1,
                    float* grad_gamma, float* grad_beta, float* grad_w2, float* grad_b2, void* workspace,
                    size_t workspace_bytes, cl3d_stream_t stream);
 

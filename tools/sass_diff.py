@@ -2,6 +2,8 @@
 
 Dumps both with `cuobjdump -sass`, drops the /*address*/ prefixes and the encoding comments, and prints the kernels
 found in only one file and the kernels whose instruction text differs, with the instruction count on each side.
+A kernel found in only one file whose instruction text equals that of a kernel found only in the other is listed as
+renamed (a template parameter added to a kernel renames its existing instance without changing its code).
 Exit status 0 when every kernel present in both files is identical, 1 otherwise."""
 import re
 import subprocess
@@ -33,6 +35,15 @@ def main(old_path, new_path):
     only_old = sorted(k for k in old if k not in new)
     only_new = sorted(k for k in new if k not in old)
     differ = sorted(k for k in old if k in new and old[k] != new[k])
+    by_code = {}
+    for k in only_new:
+        by_code.setdefault(tuple(new[k]), []).append(k)
+    renamed = [(k, by_code[tuple(old[k])].pop(0)) for k in only_old if by_code.get(tuple(old[k]))]
+    only_old = [k for k in only_old if k not in {a for a, _ in renamed}]
+    only_new = [k for k in only_new if k not in {b for _, b in renamed}]
+    print(f"renamed, same instructions: {len(renamed)}")
+    for a, b in renamed:
+        print(f"  {names[a]}  ->  {names[b]}")
     for title, ks in ((f"only in {old_path}", only_old), (f"only in {new_path}", only_new)):
         print(f"{title}: {len(ks)}")
         for k in ks:
